@@ -1,22 +1,19 @@
 # Convenience targets (everything here also works as the plain command shown).
 PY ?= python
 
-build:            ## compile the sm_100a extension in-tree (nvcc cross-compiles without a GPU)
+build:            ## compile the sm_90a extension in-tree (nvcc cross-compiles without a GPU)
 	$(PY) -m mlx_sharding_b200.ops.build
 
 test:             ## CPU test suite (models vs HF, engine, gloo chains, expert parallelism over gloo, gRPC, HTTP API, CLIs)
 	$(PY) -m pytest tests -q -m "not gpu"
 
-test-gpu:         ## on a B200 box: kernels vs fp32 oracles, models, multi-GPU parity
+test-gpu:         ## on an H100: kernels vs fp32 oracles, models, multi-GPU parity
 	$(PY) -m pytest tests -q -m gpu
 
 bench:            ## headline benchmark on 1 GPU (see bench.py for N > 1 under torchrun)
 	$(PY) bench.py
 
-sass:             ## regenerate profiles/sass_summary.md, ptxas_summary.md and the SASS excerpts from the built extension
-	$(PY) scripts/sass_summary.py
-
-harness:          ## standalone tcgen05 GEMM test binaries (no torch)
+harness:          ## standalone GEMM test binaries (no torch)
 	bash tests/cuda/build.sh
 
-.PHONY: build test test-gpu bench sass harness
+.PHONY: build test test-gpu bench harness

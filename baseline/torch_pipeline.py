@@ -1,7 +1,7 @@
 """Same-box baseline arm: the reference pipeline re-implemented as plain PyTorch (BASELINE.md §1).
 
 What the reference does (shard/utils.py:156-186, server/server.py:27-48, generate.py:52-88): layer-range pipeline stages, one
-hidden-state hand-off per stage per token, sampling after the last stage.  MLX-Metal cannot run on a B200, so this module is the
+hidden-state hand-off per stage per token, sampling after the last stage.  MLX-Metal cannot run on an H100, so this module is the
 "straight re-implementation" BASELINE.md names — and it is deliberately a *strong* one, not a strawman:
 
 * every GEMM is cuBLAS (``F.linear`` / ``torch.bmm`` on bf16), attention is ``F.scaled_dot_product_attention`` over a contiguous
@@ -469,7 +469,7 @@ def run(args, world: int, rank: int, local: int, dev, steps: Optional[int] = Non
     if rank != 0:
         return None
     return {
-        "metric": "decode tokens/sec, DeepSeek-Coder-V2-Lite @N B200, + p50 TTFT",
+        "metric": "decode tokens/sec, DeepSeek-Coder-V2-Lite @N H100, + p50 TTFT",
         "value": round(tok_s, 1), "unit": "tokens/s", "n_gpus": world, "steps": steps, "warmup": warmup,
         "ms_per_step": round(ms, 4), "higher_is_better": True, "scaling": "weak", "vs_baseline": 1.0, "dtype": "bf16",
         "data": "synthetic prompts, random-init weights", "impl": "baseline",
@@ -478,7 +478,7 @@ def run(args, world: int, rank: int, local: int, dev, steps: Optional[int] = Non
                    "tokens_per_step": G * B, "transport": "nccl send/recv" if world > 1 else "local",
                    "cuda_graphs": pipe.use_graphs, "weights": "bf16",
                    "kernels": "cuBLAS (F.linear, torch.bmm padded expert batches), F.scaled_dot_product_attention, eager elementwise",
-                   "l2": "weights streamed per step far exceed the 126 MB L2; no explicit flush",
+                   "l2": "weights streamed per step far exceed the 50 MB L2; no explicit flush",
                    "layers": "cost-balanced whole layers"},
         "ttft_p50_ms": round(ttft_p50 * 1e3, 3), "ttft_microbatch_ms": round(ttft_batch * 1e3, 2),
         "clocks": clocks.summary(), "gpu_launches": 0, "e2e": e2e_res,

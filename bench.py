@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Headline benchmark (BASELINE.json): decode tokens/sec (+ p50 TTFT) of DeepSeek-Coder-V2-Lite on N B200s.
+"""Headline benchmark (BASELINE.json): decode tokens/sec (+ p50 TTFT) of DeepSeek-Coder-V2-Lite on N H100s.
 
-    python bench.py --gpus 1 --steps 32 --warmup 4
+    python bench.py --gpus 1 --steps 32 --warmup 4 [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N --master-addr 127.0.0.1 --master-port P \
         bench.py --gpus N --steps K --warmup W
 
@@ -19,6 +19,8 @@
 * e2e     : the same metric through the public serving API (``LLMEngine.submit/step``): every step copies
             the step's token ids + metadata host->device from pinned memory and reads the sampled tokens
             back device->host.
+* --dump-outputs DIR : write the last timed step's logits and sampled token ids per group as DIR/<name>.npy (pp only, seeded
+            inputs, at most 64 MB: see ``dump_outputs``), so two builds can be compared output for output.
 * --impl reference : the unmodified mzbac/mlx_sharding from ``baseline/_ref`` (needs Apple's ``mlx``; reports
             ``unavailable`` on this platform).  --impl baseline : the same pipeline as plain PyTorch ops
             (cuBLAS GEMMs, eager, NCCL p2p hand-off) — the "straight re-implementation" BASELINE.md names.
@@ -51,7 +53,7 @@ def parse_args(argv=None):
     p.add_argument("--quant", type=int, default=0, choices=[0, 4, 8],
                    help="MLX affine quantised weights (group 64), dequantised inside the GEMM kernels (BASELINE config 2)")
     p.add_argument("--fp8-experts", action="store_true",
-                   help="convert the routed / shared expert banks to block-scaled MXFP8 at load (tcgen05 kind::mxf8f6f4); this is the "
+                   help="convert the routed / shared expert banks to block-scaled MXFP8 at load (wgmma e4m3 + per-block scales); this is the "
                         "default for --quant 4/8 checkpoints (MLXB200_FP8_EXPERTS=0 keeps the exact in-kernel MLX-affine dequant)")
     p.add_argument("--no-e2e", action="store_true")
     p.add_argument("--no-baseline", action="store_true",
@@ -59,6 +61,8 @@ def parse_args(argv=None):
     p.add_argument("--baseline-steps", type=int, default=8)
     p.add_argument("--no-graphs", action="store_true")
     p.add_argument("--page-size", type=int, default=64)
+    p.add_argument("--dump-outputs", type=str, default=None, metavar="DIR",
+                   help="write the last timed step's outputs as DIR/<name>.npy")
     p.add_argument("--whole-layers", action="store_true", help="stage boundaries only between layers (reference-style split)")
     p.add_argument("--parallelism", type=str, default="auto", choices=["auto", "pp", "ep"],
                    help="auto (default): pp on 1 GPU / dense models; on N>1 GPUs with an MoE model measure pp AND ep and headline the "
@@ -142,6 +146,11 @@ def main(argv=None):
             dist.destroy_process_group()
         return 0
 
+    ep_possible = world > 1 and args.model != "llama3-8b" and args.impl == "ours"
+    if args.dump_outputs and ep_possible and (args.parallelism == "ep" or (args.parallelism == "auto" and not args.quant)):
+        print("--dump-outputs writes the layer-range pipeline's outputs only: add --parallelism pp", file=sys.stderr)
+        return 2
+
     # a short run of the baseline arm in the same process, on the same GPUs, right before the product: fills ``vs_baseline``
     base = None
     if not args.no_baseline:
@@ -201,12 +210,12 @@ def main(argv=None):
 def weights_desc(args) -> str:
     fp8 = os.environ.get("MLXB200_FP8_EXPERTS", "")
     if args.quant:
-        exp = "expert banks converted to block-scaled MXFP8 at load (tcgen05 kind::mxf8f6f4)" if fp8 != "0" else "expert banks dequantised in-kernel"
+        exp = "expert banks converted to block-scaled MXFP8 at load (wgmma e4m3 + per-block scales)" if fp8 != "0" else "expert banks dequantised in-kernel"
         return f"mlx-affine-int{args.quant}-g64 checkpoint: attention / dense weights dequantised in-kernel, {exp}"
     return "bf16" + (", expert banks converted to block-scaled MXFP8 at load" if fp8 == "1" else "")
 
 
-METRIC = "decode tokens/sec, DeepSeek-Coder-V2-Lite @N B200, + p50 TTFT"
+METRIC = "decode tokens/sec, DeepSeek-Coder-V2-Lite @N H100, + p50 TTFT"
 
 
 def attach_baseline(res, base):
@@ -249,6 +258,30 @@ def merge_results(pp, ep):
     return dict(pp, also_measured={"expert parallel (config 5)": brief(ep)})
 
 
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir, logits, tokens):
+    """Write each group's logits [B, V] (fp32) and the token ids its step sampled (float64) to ``out_dir``.  When the logits
+    exceed the budget, every logits array keeps the same fixed, seeded, sorted subset of vocabulary columns
+    (``logits_columns.npy``)."""
+    import numpy as np
+
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {k: v.float().cpu().numpy() for k, v in logits.items()}
+    total = sum(a.size * 4 for a in arrays.values())
+    cols = None
+    if total > DUMP_LIMIT_BYTES - (1 << 20):
+        V = next(iter(arrays.values())).shape[-1]
+        keep = int(V * (DUMP_LIMIT_BYTES - (1 << 20)) / total)
+        cols = np.sort(np.random.default_rng(0).choice(V, size=keep, replace=False))
+        np.save(os.path.join(out_dir, "logits_columns.npy"), cols.astype(np.float64))
+    for k, a in arrays.items():
+        np.save(os.path.join(out_dir, k + ".npy"), a if cols is None else np.ascontiguousarray(a[:, cols]))
+    for k, t in tokens.items():
+        np.save(os.path.join(out_dir, k + ".npy"), t.cpu().numpy().astype(np.float64))
+
+
 def run_pp(args, world, rank, local, dev):
     """Layer-range pipeline: one stage per GPU, one micro-batch group per stage in flight, fused P2P hand-off."""
     import torch
@@ -273,7 +306,7 @@ def run_pp(args, world, rank, local, dev):
     else:
         from mlx_sharding_b200.ops import b200
 
-        b200.load_extension()  # fail loudly if the sm_100a extension is missing
+        b200.load_extension()  # fail loudly if the sm_90a extension is missing
 
     cfgd = model_config(args.model, args.layers)
     cfg = ModelConfig.from_dict(cfgd)
@@ -390,6 +423,9 @@ def run_pp(args, world, rank, local, dev):
     if world > 1:
         dist.barrier()
     ms = max_over_ranks(e0.elapsed_time(e1))
+    if args.dump_outputs and rank == world - 1:
+        dump_outputs(args.dump_outputs, {f"logits_g{g}": loop._outs[g] for g in range(G)},
+                     {f"tokens_g{g}": loop._toks[g] for g in range(G)})
     loop.drain()
     p2p_err = bool(loop.p2p.error()) if loop.p2p is not None else False
     launches = (loop.launches_per_step * G * args.steps) if loop.use_graphs else ((C.launch_count() - n_launch0) if C else 0)
@@ -416,7 +452,7 @@ def run_pp(args, world, rank, local, dev):
                        "micro_batches_in_flight": G, "tokens_per_step": G * B, "transport": loop.transport,
                        "cuda_graphs": loop.use_graphs, "kv_page_size": PS,
                        "weights": weights_desc(args),
-                       "l2": "weights streamed per step (31 GB/stage-set) far exceed the 126 MB L2; no explicit flush",
+                       "l2": "weights streamed per step (31 GB/stage-set) far exceed the 50 MB L2; no explicit flush",
                        "layers": [spec.start_layer, spec.end_layer] if world == 1 else
                        ("cost-balanced, whole layers" if args.whole_layers else "cost-balanced, half-layer (attention | MLP) boundaries")},
             "ttft_p50_ms": (e2e or {}).get("ttft_p50_ms") or round(ttft_p50 * 1e3, 3),
@@ -581,7 +617,7 @@ def run_ep(args, world, rank, local, dev):
                        "global_batch": world * B, "seq_len": S, "parallelism": f"ep{world}+dp{world}",
                        "tokens_per_step": world * B, "transport": "fused all-to-all over NVLink peer memory (ops/csrc/ep.cu)",
                        "cuda_graphs": loop.use_graphs, "kv_page_size": PS, "weights": "bf16",
-                       "l2": "weights streamed per step far exceed the 126 MB L2; no explicit flush"},
+                       "l2": "weights streamed per step far exceed the 50 MB L2; no explicit flush"},
             "ttft_p50_ms": (e2e or {}).get("ttft_p50_ms") or round(ttft_p50 * 1e3, 3),
             "ttft_note": f"p50 over {TTFT_REQUESTS} requests per rank through LLMEngine.submit (one {S}-token prompt at a time, all ranks in lockstep); "
                          f"ttft_stage_chain_ms = raw stage.forward",

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Expert-bank GEMM microbenchmark: block-scaled FP8 (tcgen05 kind::mxf8f6f4, ops/csrc/gemm_fp8.cu) vs bf16 (gemm_persistent.cu) on
+"""Expert-bank GEMM microbenchmark: block-scaled FP8 (wgmma e4m3 + block scales, ops/csrc/gemm_fp8.cu) vs bf16 (gemm_persistent.cu) on
 the DeepSeek-V2-Lite MoE block of a decode step (66 experts incl. the appended shared ones, 64 tokens x 8 pairs, scatter layout).
 CUDA-event timed, L2 flushed between iterations; GB/s = weight bytes / time against MEASURED_PEAKS.json."""
 import json
@@ -37,7 +37,7 @@ def main():
     try:
         hbm = json.load(open(os.path.join(root, "MEASURED_PEAKS.json")))["hbm_gbs"] * 1e9
     except Exception:  # noqa: BLE001
-        hbm = 6650e9
+        hbm = 3350e9
     E, H, I, T, k, stride = 66, 2048, 1408, 64, 8, 64
     g = torch.Generator(device=dev).manual_seed(0)
     rnd = lambda *s, sc=0.03: (torch.randn(*s, device=dev, generator=g) * sc).to(torch.bfloat16)

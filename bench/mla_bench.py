@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Decode-attention microbenchmark: absorbed-latent MLA on tcgen05 (ops/csrc/mla_decode.cu, 576-dim latent cache) vs the
+"""Decode-attention microbenchmark: absorbed-latent MLA on wgmma (ops/csrc/mla_decode.cu, 576-dim latent cache) vs the
 decompressed-cache split-KV kernel (ops/csrc/attention.cu, 16 heads x (192 + 128) per token) on DeepSeek-V2-Lite shapes.
 CUDA-event timed, L2 flushed between iterations, reports microseconds and achieved KV bytes/s against MEASURED_PEAKS.json."""
 import json
@@ -37,7 +37,7 @@ def main():
         hbm = json.load(open(os.path.join(root, "MEASURED_PEAKS.json")))["hbm_gbs"] * 1e9
         basis = "measured"
     except Exception:  # noqa: BLE001
-        hbm, basis = 6650e9, "fallback"
+        hbm, basis = 3350e9, "fallback"
     out = {"bench": "decode attention, DeepSeek-V2-Lite shapes (16 heads), B sequences x ctx tokens", "hbm_basis": f"{basis} {hbm / 1e9:.0f} GB/s",
            "rows": []}
     scale = 192 ** -0.5

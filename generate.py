@@ -27,7 +27,7 @@ def build_engine(model, server_address, num_pages=None, page_size=64):
     stage = StageExecutor(model, num_pages, page_size)
     world = int(os.environ.get("WORLD_SIZE", "1"))
     if world > 1:
-        # native chain: shared-memory launch ring + fused P2P hand-off on B200 (gloo / NCCL send-recv elsewhere)
+        # native chain: shared-memory launch ring + fused P2P hand-off on CUDA (gloo / NCCL send-recv elsewhere)
         return LLMEngine(ChainPipeline.build(stage, num_groups=1, max_tokens=2048, max_seqs=64), num_pages, page_size,
                          num_groups=1, max_prefill_tokens=2048)
     if not model.spec.is_last:

@@ -3,13 +3,13 @@
 Reference: ``shard/server/model/deepseek_v2.py`` (layer-range wrapper, expert stacking at :101-111,
 tuple ``head_dim`` = (192, 128) at :120-125) + upstream ``DeepseekV2DecoderLayer`` (SURVEY U3, §3.6).
 
-B200 design notes:
+Design notes:
 * ``q_proj`` and ``kv_a_proj_with_mqa`` are concatenated at load into one GEMM (SURVEY K3/K4) when the
   model has no q-LoRA (DeepSeek-V2-Lite);
 * the KV cache keeps the reference's *decompressed* layout (K 192 / V 128 per head) so results are
   bit-comparable with the reference pipeline; the MLA append kernel assembles ``[k_nope | k_pe]``
   straight into the paged pool;
-* MoE = router kernel (fp32 softmax + top-k) -> token permutation -> grouped swap-AB tcgen05 GEMMs over
+* MoE = router kernel (fp32 softmax + top-k) -> token permutation -> grouped swap-AB wgmma GEMMs over
   the stacked ``switch_mlp`` weights -> weighted combine fused with shared-expert output + residual.
 """
 from __future__ import annotations
@@ -32,7 +32,7 @@ class DeepseekV2Stage(StageModel):
     # KV layout: cache the 512-dim latent + the 64-dim roped key (one shared "head", 576 values per token) instead of the
     # reference's decompressed per-head K/V (16 x (192 + 128) = 5120 values, shard/server/model/deepseek_v2.py:120-125) and absorb
     # kv_b into the query / output side.  Mathematically identical attention (see ``_attn_absorbed``).
-    #   None (default): automatic — on when the sm_100a latent-attention kernel supports the shapes (16 heads, kv_lora_rank 512,
+    #   None (default): automatic — on when the sm_90a latent-attention kernel supports the shapes (16 heads, kv_lora_rank 512,
     #                   rope 64, no q-LoRA, unquantised attention weights, 64-token pages: DeepSeek-V2-Lite / Coder-V2-Lite);
     #   MLXB200_ABSORBED_MLA=0 / 1 forces it off / on (``1`` on the reference backend selects the einsum formulation).
     absorbed_mla = {"0": False, "1": True}.get(os.environ.get("MLXB200_ABSORBED_MLA", ""), None)
@@ -58,7 +58,7 @@ class DeepseekV2Stage(StageModel):
     def kv_geometry(self):
         if self.absorbed_mla:
             c = self.cfg
-            # the sm_100a kernel reads the values as the first 512 dims of the cached key row (no second pool)
+            # the sm_90a kernel reads the values as the first 512 dims of the cached key row (no second pool)
             dv = 0 if self.backend_name == "b200" else c.kv_lora_rank
             return self.spec.num_kv_layers, 1, c.kv_lora_rank + c.qk_rope_head_dim, dv
         return super().kv_geometry()
@@ -161,7 +161,7 @@ class DeepseekV2Stage(StageModel):
         normed = pn[1] if (pn is not None and pn[0] is h) else O.rmsnorm(h, w["in_ln"], c.rms_norm_eps)
         if "qkv_abs" in w and meta.max_q_len == 1 and meta.num_tokens == meta.num_seqs and kpool.shape[2] == 64:
             # decode step on the absorbed weights: one GEMM -> [q_abs | q_pe] x 16 heads, c_kv, k_pe; fused prologue (latent norm,
-            # both ropes, cache append); tcgen05 multi-query attention over the cached latent; folded output projection
+            # both ropes, cache append); wgmma multi-query attention over the cached latent; folded output projection
             qkv = O.linear(normed, w["qkv_abs"])
             if self.backend_name == "b200" and "router" in w and w.get("e_gate") is not None and not w["e_gate"].is_quantized \
                     and not O.fp8_experts_enabled(w["e_gate"]):
@@ -226,8 +226,8 @@ class DeepseekV2Stage(StageModel):
         keeps every weight packed and dequantised in-kernel with exact MLX-affine semantics):
 
         * routed + shared expert banks (93 % of the parameters) -> block-scaled MXFP8 (``utils/quant.py::to_mxfp8``), executed by
-          ``tcgen05.mma kind::mxf8f6f4.block_scale`` (``ops/csrc/gemm_fp8.cu``); the shared experts are appended to the bank first;
-        * attention projections (7 %) -> bf16, so the absorbed-latent MLA path (folded weights, tcgen05 latent attention) applies;
+          wgmma e4m3 with per-32 block scales (``ops/csrc/gemm_fp8.cu``); the shared experts are appended to the bank first;
+        * attention projections (7 %) -> bf16, so the absorbed-latent MLA path (folded weights, wgmma latent attention) applies;
         * embeddings, LM head, dense layer-0 MLP stay packed (in-kernel dequant GEMMs / gather).
 
         With MLXB200_FP8_EXPERTS=1 the expert banks of a bf16 checkpoint are converted the same way."""
@@ -306,7 +306,7 @@ class DeepseekV2Stage(StageModel):
         """Prefill chunk / mixed batch with the latent cache (CUDA backend): append this chunk's latents, then *decompress the
         context the batch attends to* (``kv_b`` GEMM over the cached latents of its sequences) into a temporary per-head K/V pool
         and run the tensor-core flash-prefill kernel on it.  Costs O(context) extra GEMM work per chunk, prefill only; decode steps
-        never come here (``attn_block`` routes them to the tcgen05 latent kernel)."""
+        never come here (``attn_block`` routes them to the wgmma latent kernel)."""
         O, c = self.ops, self.cfg
         T = h.shape[0]
         nh, nope, rd, vd, lr = c.num_attention_heads, c.qk_nope_head_dim, c.qk_rope_head_dim, c.v_head_dim, c.kv_lora_rank

@@ -3,8 +3,8 @@
 Reference: ``shard/server/model/llama.py`` (layer-range wrapper) + upstream ``TransformerBlock``
 (SURVEY U1): pre-norm block, GQA, half-split RoPE with optional linear / llama3 scaling, SwiGLU MLP.
 
-B200 design: Q/K/V projections are concatenated at load into one ``[Nq+2Nkv, H]`` weight (one GEMM
-launch, SURVEY K3/K4); gate/up run as one dual-accumulator tcgen05 GEMM with the SiLU·mul epilogue;
+Design: Q/K/V projections are concatenated at load into one ``[Nq+2Nkv, H]`` weight (one GEMM
+launch, SURVEY K3/K4); gate/up run as one dual-accumulator wgmma GEMM with the SiLU·mul epilogue;
 residual adds ride the O-proj / down-proj GEMM epilogues; the last down-proj of a stage is the kernel
 that stores straight into the next stage's input buffer (``parallel/p2p_fused.py``).
 """

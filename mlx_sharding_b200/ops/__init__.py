@@ -1,7 +1,7 @@
 """Op API.  Two interchangeable implementations of the same function set:
 
 * ``reference`` – pure PyTorch (CPU path, numerical oracle, and — on CUDA tensors — the cuBLAS baseline)
-* ``b200``      – hand-written sm_100a CUDA kernels (``ops/csrc``; tcgen05/TMEM/TMA GEMMs, paged flash
+* ``b200``      – hand-written sm_90a CUDA kernels (``ops/csrc``; wgmma/TMA GEMMs, paged flash
                   attention, MoE, sampler, fused P2P stage boundary)
 
 There is no silent fallback: asking for ``b200`` on a box whose extension is missing raises.

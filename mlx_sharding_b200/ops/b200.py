@@ -1,4 +1,4 @@
-"""``b200`` op backend: the hand-written sm_100a kernels behind the same API as ``ops.reference``.
+"""``b200`` op backend: the hand-written sm_90a kernels behind the same API as ``ops.reference``.
 
 Loading is strict: if the extension is missing (or is not loadable) on a box with a GPU this raises —
 there is no silent PyTorch fallback on the hot path.  The only non-kernel code here is argument
@@ -35,7 +35,7 @@ def load_extension(build_if_missing: bool = False):
             build()
         else:
             raise ImportError(
-                f"{_SO} not found: build the sm_100a extension with `python -m mlx_sharding_b200.ops.build` "
+                f"{_SO} not found: build the sm_90a extension with `python -m mlx_sharding_b200.ops.build` "
                 "(or __graft_entry__.build())")
     spec = importlib.util.spec_from_file_location("_b200_C", _SO)
     mod = importlib.util.module_from_spec(spec)
@@ -402,7 +402,7 @@ def moe_block(x, gate_w, route_kw: dict, Wg: LinearWeight, Wu: LinearWeight, Wd:
     k = idx.shape[1]
     if fp8:
         # block-scaled FP8 experts: activations are quantised per 32-wide K block right before each GEMM (garbage rows beyond an
-        # expert's count are quantised too and never read); tcgen05 kind::mxf8f6f4.block_scale applies both operands' scales
+        # expert's count are quantised too and never read); the FP8 GEMM applies both operands' block scales
         xq, xsf = c.quant_mxfp8(xs)
         h = c.linear_fp8(xq, xsf, gq, gs, uq, us, counts, stride, None, ACT_IDS[act], False, T * k, stride)
         hq, hsf = c.quant_mxfp8(h)
@@ -442,7 +442,7 @@ def sample(logits, temperature, top_p, generator: Optional[torch.Generator] = No
 
 
 def mla_absorbed_supported(num_heads: int, kv_lora_rank: int, rope_dim: int, page_size: int = 64) -> bool:
-    """Shapes the tcgen05 absorbed-latent MLA decode kernel is built for (DeepSeek-V2 / V2-Lite / Coder-V2-Lite)."""
+    """Shapes the wgmma absorbed-latent MLA decode kernel is built for (DeepSeek-V2 / V2-Lite / Coder-V2-Lite)."""
     return num_heads == 16 and kv_lora_rank == 512 and rope_dim == 64 and page_size == 64
 
 
@@ -452,7 +452,7 @@ def mla_absorbed_prologue(q, ckv, k_pe, norm_w, eps: float, pool, meta: BatchMet
 
 
 def mla_decode(q, pool, meta: BatchMeta, scale: float, nsplit: int = 0):
-    """Multi-query attention over the cached latent (d_qk 576 / d_v 512) on tcgen05: ``[B, 16, 576] -> [B, 16, 512]``."""
+    """Multi-query attention over the cached latent (d_qk 576 / d_v 512) on wgmma: ``[B, 16, 576] -> [B, 16, 512]``."""
     return C().mla_decode(q, pool, meta.block_tables, meta.context_lens, float(scale), int(meta.max_ctx_len), int(nsplit))
 
 

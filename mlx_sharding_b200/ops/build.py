@@ -1,9 +1,9 @@
-"""In-tree build of the sm_100a extension (``mlx_sharding_b200/ops/_b200_C.so``).
+"""In-tree build of the sm_90a (H100) extension (``mlx_sharding_b200/ops/_b200_C.so``).
 
 Kernel sources are plain CUDA (no torch headers) compiled by nvcc with
-``-gencode arch=compute_100a,code=sm_100a -lineinfo``; only ``bindings.cpp`` sees torch.  nvcc
-cross-compiles without a GPU, so this runs on the CPU build box; the resulting ``.so`` travels to the
-GPU box with the repo snapshot (it is git-ignored, not gpurun-ignored).
+``-gencode arch=compute_90a,code=sm_90a -lineinfo``; only ``bindings.cpp`` sees torch.  nvcc
+cross-compiles without a GPU, so the extension can be built on a machine without one; the ``.so`` and
+the object directory are git-ignored build products.
 
 ``python -m mlx_sharding_b200.ops.build [--force] [--verbose]``
 """
@@ -23,7 +23,7 @@ MODULE = "_b200_C"
 SO_PATH = os.path.join(HERE, MODULE + ".so")
 
 CU_SOURCES = ["gemm_tcgen05.cu", "gemm_persistent.cu", "gemm_q_tcgen05.cu", "gemm_q_persistent.cu", "gemm_fp8.cu", "elementwise.cu", "attention.cu", "attention_prefill.cu", "mla_decode.cu", "moe.cu", "sampler.cu", "p2p.cu", "ep.cu"]
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ARCH + ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "--use_fast_math",
                      "-Xptxas", "-v"]
 

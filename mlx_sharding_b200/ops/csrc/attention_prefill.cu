@@ -9,8 +9,8 @@
 // double buffered with cp.async straight from the page pool into padded (bank-conflict-free) shared memory.
 // S = QK^T and O += PV run on the tensor cores through warp-level mma.m16n8k16 (bf16 in, fp32 accumulate) with
 // the FA-2 register pipeline (S accumulators are re-used as the A operand of PV); softmax is online in
-// registers with exp2.  NOTE: this is the legacy (HMMA) tensor path — the tcgen05/TMEM version of this
-// kernel is the planned replacement; the GEMMs that dominate prefill FLOPs already run on tcgen05.
+// registers with exp2.  NOTE: this is the legacy (HMMA) tensor path — a wgmma version of this
+// kernel is the planned replacement; the GEMMs that dominate prefill FLOPs already run on wgmma.
 #include "kernels.h"
 #include "launch.h"
 #include "ptx.cuh"

@@ -1,4 +1,4 @@
-// PyTorch bindings for the sm_100a kernels.  Everything launches on the current torch CUDA stream so
+// PyTorch bindings for the sm_90a kernels.  Everything launches on the current torch CUDA stream so
 // the ops compose with torch.cuda.CUDAGraph capture; scratch buffers are process-lifetime (never freed,
 // never moved once handed to a kernel) so captured graphs stay valid.
 #include <ATen/cuda/CUDAContext.h>
@@ -72,9 +72,8 @@ int sm_count() {
   return n;
 }
 
-// Token tile of the grouped (MoE) GEMMs: ~2x the average rows per expert but never below 64 — measured on B200
-// (profiles/results.md, DeepSeek-V2-Lite decode): tiles of 16 / 32 tokens are *slower* than 64 even when experts hold ~6
-// rows, and 256-token tiles lose to 64 / 128 at 24 rows per expert.  MLXB200_GROUPED_BN=<n> overrides (tuning).
+// Token tile of the grouped (MoE) GEMMs: ~2x the average rows per expert but never below 64, so an expert's rows rarely need a
+// second tile; gemm_clamp_bn caps it at what the register accumulators allow.  MLXB200_GROUPED_BN=<n> overrides (tuning).
 int grouped_bn(int64_t max_rows, int64_t R, int64_t E) {
   static const int forced = [] { const char* e = std::getenv("MLXB200_GROUPED_BN"); return e ? std::atoi(e) : 0; }();
   if (forced > 0) return b200::gemm_pick_bn((int)std::min<int64_t>(max_rows, forced));
@@ -86,7 +85,7 @@ int auto_splits(int rows, int n, int k, bool grouped) {
   const int tiles = (n + 127) / 128;
   const int kb = (k + 63) / 64;
   int s = 1;
-  // fill ~one wave of SMs while keeping >= 8 k-blocks per split (measured: profiles/splitk_sweep.md) ...
+  // fill ~one wave of SMs while keeping >= 8 k-blocks per split ...
   while (tiles * (s * 2) <= sm_count() && kb / (s * 2) >= 8 && s < 4) s *= 2;
   // ... and for long reductions over few feature tiles (the folded MLA output projection: 16 tiles x 128 k-blocks) go to the
   // full portable cluster of 8 splits: 64 CTAs stream at ~100 GB/s each, so the kernel is per-SM-bandwidth bound below that
@@ -797,7 +796,7 @@ Tensor ep_combine(int64_t flag_ptr, const Tensor& expected, int64_t error_ptr, c
 }  // namespace
 
 PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
-  m.doc() = "mlx_sharding_b200 sm_100a kernels";
+  m.doc() = "mlx_sharding_b200 sm_90a kernels";
   m.def("linear", &linear, py::arg("x"), py::arg("w"), py::arg("w2") = py::none(), py::arg("residual") = py::none(),
         py::arg("bias") = py::none(), py::arg("act") = 0, py::arg("softcap") = 0.0, py::arg("out_fp32") = false,
         py::arg("out") = py::none(), py::arg("splits") = 0, py::arg("signal_flag_ptr") = 0, py::arg("signal_value") = 0);
@@ -869,5 +868,5 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("init_scratch", &init_scratch);
   m.def("launch_count", []() { return g_launches; });
   m.def("pdl_skip_next", []() { b200::pdl_skip_next(); });
-  m.def("sm_arch", []() { return std::string("sm_100a"); });
+  m.def("sm_arch", []() { return std::string("sm_90a"); });
 }

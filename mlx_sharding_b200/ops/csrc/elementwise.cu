@@ -2,7 +2,7 @@
 // with in-kernel MLX-affine dequant, RMSNorm (+Gemma variant, + post-norm residual), rotary embedding
 // (half-split and interleaved/YaRN), paged KV-cache append (plain and MLA-assembling).
 // The reference gets all of these from MLX Metal kernels (mx.fast.rms_norm / mx.fast.rope / Embedding /
-// KVCache.update_and_fetch via mlx_lm blocks); these are from-scratch sm_100a kernels: 128-bit
+// KVCache.update_and_fetch via mlx_lm blocks); these are from-scratch sm_90a kernels: 128-bit
 // vectorised accesses, one warp-shuffle reduction tree, no shared-memory round trips beyond one exchange.
 #include <cuda_fp8.h>
 
@@ -252,7 +252,7 @@ __global__ void embed_quant_kernel(const long long* __restrict__ ids, const uint
 }
 
 // ------------------------------------------------------------------------------------------------ L2 prefetch
-// Pulls a weight range into the 126 MB L2 with bulk prefetches (no SM registers / shared memory involved, a handful of threads).
+// Pulls a weight range into the 50 MB L2 with bulk prefetches (no SM registers / shared memory involved, a handful of threads).
 // Launched on a side stream while the latency-bound attention chain of a decode layer leaves HBM idle, for the first experts of the
 // MoE bank the following grouped GEMM streams: that GEMM is HBM-bound, so every byte already in L2 comes off its critical path.
 __global__ void l2_prefetch_kernel(const char* __restrict__ p, unsigned long long bytes) {

@@ -9,7 +9,7 @@
 //               source pair) record; the last CTA publishes (row count << 32 | step sequence) to each destination
 //               as one 64-bit st.release.sys.
 //   regroup   : the destination polls the W words (ld.acquire.sys), buckets what it received by local expert
-//               (offsets + gather) so the swap-AB grouped tcgen05 GEMMs run on contiguous rows, and records for
+//               (offsets + gather) so the swap-AB grouped GEMMs run on contiguous rows, and records for
 //               every row the address of its slot in the source rank's return buffer.
 //   return    : there is no return kernel — the grouped down-projection's epilogue (gemm_persistent.cu, GemmParams::
 //               row_dst / signal_peers) stores each fp32 output row straight to that address and the CTA completing the

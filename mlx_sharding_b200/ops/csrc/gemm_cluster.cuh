@@ -1,10 +1,10 @@
 // Split-K reduction through distributed shared memory (thread-block cluster), used for decode-shaped GEMMs.
 //
-// With few output tiles (N/128 = 16..32) a skinny GEMM cannot fill 148 SMs unless K is split, but reducing the
-// partials through global memory (workspace + fence + ticket + re-read) costs more than the GEMM itself
-// (measured ~7 us on top of a ~7 us kernel, profiles/splitk_sweep.md).  Here the `splits` CTAs that share an
+// With few output tiles (N/128 = 16..32) a skinny GEMM cannot fill 132 SMs unless K is split, but reducing the
+// partials through global memory (workspace + fence + ticket + re-read) costs about as much as the decode GEMM itself.
+// Here the `splits` CTAs that share an
 // output tile form one cluster (cluster dims {1,1,splits}):
-//   phase A  every CTA drains its TMEM accumulator into its *own* shared memory as fp32 [cols][128];
+//   phase A  every CTA stores its register accumulator into its *own* shared memory as fp32 [cols][128];
 //   barrier.cluster (release/acquire);
 //   phase B  CTA r sums token columns [r*BN/S, (r+1)*BN/S) over all S CTAs with ld.shared::cluster (DSMEM),
 //            in split order (deterministic), applies the epilogue and stores its rows;
@@ -35,33 +35,7 @@ B200_DEVICE float ld_dsmem_f32(uint32_t addr) {
   return v;
 }
 
-// Phase A (epilogue warps): TMEM accumulator -> own shared memory, fp32, layout [col][128 features].
-template <int BN, bool DUAL>
-__device__ __forceinline__ void cluster_epilogue_store_partial(uint8_t* smem, uint32_t tmem_base, uint64_t* tmem_full_bar, int warp,
-                                                               int lane, int num_kb) {
-  const int q = warp & 3;
-  const int f_local = q * 32 + lane;
-  mbar_wait(tmem_full_bar, 0);
-  tc_fence_after();
-  const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16);
-  float* part = reinterpret_cast<float*>(smem);
-#pragma unroll 1
-  for (int c = 0; c < BN * (DUAL ? 2 : 1); c += 16) {
-    uint32_t v[16];
-    if (num_kb > 0) {
-      tmem_ld16(taddr + c, v);
-      tmem_ld_wait();
-    } else {
-#pragma unroll
-      for (int j = 0; j < 16; ++j) v[j] = 0u;
-    }
-#pragma unroll
-    for (int j = 0; j < 16; ++j) part[(c + j) * kTileM + f_local] = __uint_as_float(v[j]);
-  }
-  tc_fence_before();
-}
-
-// Phase B (epilogue warps): reduce this CTA's slice of token columns over the cluster, epilogue, store.
+// Phase B (MMA warpgroup): reduce this CTA's slice of token columns over the cluster, epilogue, store.
 template <int BN, bool DUAL, typename OutT>
 __device__ __forceinline__ void cluster_epilogue_reduce_store(const GemmParams& p, uint8_t* smem, int epi_base, int n0, int row_base,
                                                               int rows_valid) {

@@ -1,7 +1,7 @@
-// Shared pieces of the swap-AB tcgen05 GEMM family: tile constants and the TMEM -> registers -> shared ->
-// global epilogue (bias / activation-gating / soft-cap / residual / split-K reduction / fused P2P signal).
-// Used by the dense (TMA-fed bf16 weights, gemm_tcgen05.cu) and the quantised (in-kernel MLX-affine
-// dequant, gemm_q_tcgen05.cu) kernels.
+// Shared pieces of the swap-AB wgmma GEMM family: tile constants, the warpgroup main loop and the
+// registers -> shared -> global epilogue (bias / activation-gating / soft-cap / residual / split-K reduction /
+// fused P2P signal).  Used by the dense (TMA-fed bf16 weights, gemm_tcgen05.cu) and the quantised (in-kernel
+// MLX-affine dequant, gemm_q_tcgen05.cu) kernels and their persistent variants.
 #pragma once
 #include "gemm_tcgen05.h"
 #include "ptx.cuh"
@@ -9,27 +9,79 @@
 namespace b200 {
 namespace gemm {
 
-constexpr int kTileM = 128;      // output features per CTA (UMMA M)
+constexpr int kTileM = 128;      // output features per CTA (two wgmma M = 64 halves)
 constexpr int kBlockK = 64;      // bf16 elements per k-block = one 128B swizzle row
-constexpr int kUmmaK = 16;
-constexpr int kNumThreads = 192;  // warp0: TMA, warp1: MMA + TMEM alloc, warps 2..5: epilogue
+constexpr int kMmaK = 16;
+constexpr int kNumThreads = 160;  // warps 0..3: MMA warpgroup + epilogue, warp 4: TMA
 constexpr int kEpiThreads = 128;
+constexpr int kProducerWarp = 4;
 constexpr int kATileBytes = kTileM * kBlockK * 2;  // 16 KB
+// Register accumulators bound the token tile: 128 x BN fp32 over 128 threads is BN registers per weight matrix.
+constexpr int kMaxBN = 128, kMaxBNDual = 64;
 
+__host__ __device__ constexpr int acc_bytes(int BN, bool dual) { return BN * (dual ? 2 : 1) * kTileM * 4; }
 __host__ __device__ constexpr int stage_bytes(int BN, bool dual) {
   return kATileBytes * (dual ? 2 : 1) + BN * kBlockK * 2;
 }
 __host__ __device__ constexpr int num_stages(int BN, bool dual, int out_bytes) {
-  // leave room for barriers; the epilogue staging buffer aliases the (by then idle) stage ring
+  // leave room for barriers; the accumulator and the epilogue staging buffer alias the (by then idle) stage ring
   int s = (200 * 1024) / stage_bytes(BN, dual);
   s = s > 8 ? 8 : s;
-  // the ring must be at least as large as the epilogue staging tile
-  while (s * stage_bytes(BN, dual) < BN * kTileM * out_bytes) ++s;
+  while (s * stage_bytes(BN, dual) < acc_bytes(BN, dual) + BN * kTileM * out_bytes) ++s;
   return s;
 }
-__host__ __device__ constexpr uint32_t tmem_cols(int BN, bool dual) {
-  int c = BN * (dual ? 2 : 1);
-  return c <= 32 ? 32 : c <= 64 ? 64 : c <= 128 ? 128 : c <= 256 ? 256 : 512;
+
+// One k-block (64 deep) of a 128 x BN tile: two M = 64 halves of the weight tile against the token tile, both K-major.
+template <int BN>
+__device__ __forceinline__ void mma_kblock(float (&acc)[2][BN / 2], uint32_t a_addr, uint32_t b_addr) {
+  const uint64_t bdesc = gmma_desc_sw128(b_addr);
+#pragma unroll
+  for (int kk = 0; kk < kBlockK / kMmaK; ++kk)
+#pragma unroll
+    for (int h = 0; h < 2; ++h) wgmma_bf16<BN>(acc[h], gmma_desc_sw128(a_addr + h * 64 * 128) + 2 * kk, bdesc + 2 * kk);
+}
+
+template <int BN>
+__device__ __forceinline__ void acc_zero(float (&acc)[2][BN / 2]) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int j = 0; j < BN / 2; ++j) acc[h][j] = 0.f;
+}
+
+// MMA warpgroup main loop of one tile over ring iterations [it0, it0 + num_kb): `ready(stage, phase)` waits until the stage is
+// filled; a stage is released (one arrival per warp, empty barriers count 4) once the MMAs reading it have completed.
+template <int BN, bool DUAL, int STAGES, int STAGE_BYTES, int OFF_B, typename Ready>
+__device__ __forceinline__ void mma_mainloop(float (&acc)[2][BN / 2], float (&acc2)[2][BN / 2], uint8_t* smem, uint64_t* empty_bar,
+                                             uint32_t it0, int num_kb, Ready ready) {
+  const bool leader = (threadIdx.x & 31) == 0;
+  for (int i = 0; i < num_kb; ++i) {
+    const uint32_t it = it0 + i, s = it % STAGES;
+    ready(s, (it / STAGES) & 1);
+    const uint32_t a_addr = smem_u32(smem + s * STAGE_BYTES);
+    wgmma_fence();
+    mma_kblock<BN>(acc, a_addr, a_addr + OFF_B);
+    if (DUAL) mma_kblock<BN>(acc2, a_addr + kATileBytes, a_addr + OFF_B);
+    wgmma_commit();
+    wgmma_wait<1>();  // the previous k-block's MMAs are done: its stage can be refilled
+    if (i > 0 && leader) mbar_arrive(&empty_bar[(it - 1) % STAGES]);
+  }
+  wgmma_wait<0>();
+#pragma unroll
+  for (int h = 0; h < 2; ++h) {
+    wgmma_fence_acc(acc[h]);
+    if (DUAL) wgmma_fence_acc(acc2[h]);
+  }
+  if (num_kb > 0 && leader) mbar_arrive(&empty_bar[(it0 + num_kb - 1) % STAGES]);
+}
+
+// Register accumulator -> shared memory fp32 [col][128 features] (column offset `c0`: the second matrix of a DUAL pair at BN).
+template <int BN>
+__device__ __forceinline__ void acc_store_smem(const float (&acc)[2][BN / 2], float* buf, int c0) {
+#pragma unroll
+  for (int h = 0; h < 2; ++h)
+#pragma unroll
+    for (int j = 0; j < BN / 2; ++j) buf[(c0 + wg_col(j)) * kTileM + h * 64 + wg_row(j)] = acc[h][j];
 }
 
 __device__ __forceinline__ float apply_act(int act, float g) {
@@ -51,19 +103,14 @@ template <>
 __device__ __forceinline__ void stage_store<float>(float* p, float v) { *p = v; }
 
 
-// Runs on the 4 epilogue warps (threads [epi_base, epi_base + 128)); `warp` is the CTA-wide warp index.
+// Runs on the MMA warpgroup (threads [epi_base, epi_base + 128)) once the tile's accumulator is in shared memory (`acc`,
+// fp32 [col][128 features], DUAL second matrix at column BN); `stg` is the bf16 / fp32 staging tile [BN][128].
 template <int BN, bool DUAL, typename OutT>
-__device__ __forceinline__ void run_epilogue(const GemmParams& p, uint8_t* smem, uint32_t tmem_base, uint64_t* tmem_full_bar,
-                                             uint32_t* flag_smem, int warp, int lane, int epi_base, int n0, int mt, int split,
-                                             int row_base, int rows_valid, int num_kb) {
-    // ============================================================== epilogue warps (128 threads)
-    const int q = warp & 3;             // TMEM lane quarter this warp may access
-    const int f_local = q * 32 + lane;  // feature within the tile == TMEM lane
-    const int f_glob = n0 + f_local;
+__device__ __forceinline__ void run_epilogue(const GemmParams& p, const float* acc, OutT* stg, uint32_t* flag_smem, int epi_base, int n0,
+                                             int mt, int split, int row_base, int rows_valid) {
     const int et = threadIdx.x - epi_base;  // 0..127
-    mbar_wait(tmem_full_bar, 0);
-    tc_fence_after();
-    const uint32_t taddr = tmem_base + (static_cast<uint32_t>(q * 32) << 16);
+    const int f_local = et;                 // feature within the tile
+    const int f_glob = n0 + f_local;
 
     bool do_epilogue = true;
     if (p.splits > 1) {
@@ -71,18 +118,7 @@ __device__ __forceinline__ void run_epilogue(const GemmParams& p, uint8_t* smem,
       float* ws = p.workspace + (static_cast<size_t>((blockIdx.y * gridDim.x + blockIdx.x) * (gridDim.z / p.splits) + mt) *
                                  p.splits + split) * (BN * (DUAL ? 2 : 1) * kTileM);
 #pragma unroll 1
-      for (int c = 0; c < BN * (DUAL ? 2 : 1); c += 16) {
-        uint32_t v[16];
-        if (num_kb > 0) {
-          tmem_ld16(taddr + c, v);
-          tmem_ld_wait();
-        } else {
-#pragma unroll
-          for (int j = 0; j < 16; ++j) v[j] = 0u;
-        }
-#pragma unroll
-        for (int j = 0; j < 16; ++j) ws[(c + j) * kTileM + f_local] = __uint_as_float(v[j]);
-      }
+      for (int c = 0; c < BN * (DUAL ? 2 : 1); ++c) ws[c * kTileM + f_local] = acc[c * kTileM + f_local];
       __threadfence();
       named_bar_sync(1, kEpiThreads);
       if (et == 0) {
@@ -98,7 +134,6 @@ __device__ __forceinline__ void run_epilogue(const GemmParams& p, uint8_t* smem,
     }
 
     if (do_epilogue) {
-      OutT* stg = reinterpret_cast<OutT*>(smem);  // aliases the idle stage ring: [BN][128]
       const float bias = (p.bias != nullptr && f_glob < p.n) ? __bfloat162float(p.bias[f_glob]) : 0.0f;
       const float* ws0 = nullptr;
       if (p.splits > 1)
@@ -134,16 +169,10 @@ __device__ __forceinline__ void run_epilogue(const GemmParams& p, uint8_t* smem,
             }
           }
         } else {
-          uint32_t v[16];
-          tmem_ld16(taddr + c, v);
-          tmem_ld_wait();
 #pragma unroll
-          for (int j = 0; j < 16; ++j) g[j] = __uint_as_float(v[j]);
-          if (DUAL) {
-            tmem_ld16(taddr + BN + c, v);
-            tmem_ld_wait();
-#pragma unroll
-            for (int j = 0; j < 16; ++j) u[j] = __uint_as_float(v[j]);
+          for (int j = 0; j < 16; ++j) {
+            g[j] = acc[(c + j) * kTileM + f_local];
+            if (DUAL) u[j] = acc[(BN + c + j) * kTileM + f_local];
           }
         }
 #pragma unroll
@@ -154,7 +183,6 @@ __device__ __forceinline__ void run_epilogue(const GemmParams& p, uint8_t* smem,
           stage_store<OutT>(&stg[(c + j) * kTileM + f_local], y);
         }
       }
-      tc_fence_before();
       named_bar_sync(1, kEpiThreads);
       // ---- coalesced write-out: each token row of the tile is 128 features = 16 chunks of 8 elements
       constexpr int kVec = 8;
@@ -211,7 +239,6 @@ __device__ __forceinline__ void run_epilogue(const GemmParams& p, uint8_t* smem,
         }
       }
     }
-    tc_fence_before();
 }
 
 }  // namespace gemm

@@ -1,21 +1,18 @@
-// Block-scaled FP8 (MXFP8) variant of the persistent swap-AB GEMM: tcgen05.mma kind::mxf8f6f4.block_scale.
+// Block-scaled FP8 (MXFP8) variant of the persistent swap-AB GEMM on wgmma (e4m3 x e4m3, fp32 accumulate).
 //
 // SURVEY §2.6 K17 / BASELINE north star: "block-scaled fp8 where the checkpoint is 4-bit/8-bit".  MLX-affine int4/int8 weights are
 // dequantised in shared memory by gemm_q_*.cu (exact MLX semantics, but the dequant ALU work caps the speed-up); here they are
 // converted ONCE at load to OCP MXFP8 — e4m3 elements with one power-of-two (ue8m0) scale per 32 consecutive K values
-// (utils/quant.py::to_mxfp8) — and the tensor core applies both operands' block scales itself:
+// (utils/quant.py::to_mxfp8):
 //
 //   * weights [N, K] e4m3 + scales [N, K/32] ue8m0, activations [T, K] e4m3 + scales [T, K/32] (quantised by
 //     elementwise.cu::quant_mxfp8_kernel); 1 byte per element, so a 128 B swizzle row is one 128-element k-block and a stage has
-//     the same bytes as in the bf16 kernel with half the TMA / MMA instruction count per weight byte;
-//   * UMMA K = 32 per instruction = exactly one scale block: the four MMAs of a k-block select byte 0..3 (a_sf_id / b_sf_id) of the
-//     32-bit scale words staged in TMEM;
-//   * scale staging: 4 extra warps (one per TMEM lane quarter) read the scale words of the stage's rows from global memory
-//     and tcgen05.st them into the slot's TMEM columns in the layout the MMA expects (row r -> lane r % 32 of every quarter,
-//     column r / 32), ahead of the TMA ring; accumulators stay fp32 in TMEM and the epilogue is the bf16 kernel's.
+//     the same bytes as in the bf16 kernel;
+//   * wgmma K = 32 per instruction = exactly one scale block: each block's product goes to a fresh register tile that the warpgroup
+//     scales by (weight scale x token scale) and adds into the fp32 accumulator (sm_90 has no block-scaled MMA).
 //
-// Everything else — persistent tile walk, double-buffered accumulators, grouped (MoE) mode incl. the fixed-stride scatter layout,
-// DUAL gate/up with act(g)*u epilogue, residual / fp32 outputs — is shared by construction with gemm_persistent.cu.
+// Everything else — persistent tile walk, grouped (MoE) mode incl. the fixed-stride scatter layout, DUAL gate/up with act(g)*u
+// epilogue, residual / fp32 outputs — is shared by construction with gemm_persistent.cu.
 #include <algorithm>
 
 #include "gemm_common.cuh"
@@ -28,22 +25,15 @@ using namespace gemm;
 
 namespace {
 
-constexpr int kSfWarps = 4;                 // scale-staging warps per group (one per TMEM lane quarter)
-constexpr int kSfGroups = 3;                // groups take ring iterations round-robin: three global-load round trips in flight
-constexpr int kFp8Threads = kNumThreads + 32 * kSfWarps * kSfGroups;
-constexpr int kSfColsPerStage = 16;         // TMEM columns per ring slot: SFA (4, DUAL 8) + SFB (BN / 32 <= 8)
+constexpr int kFp8Threads = kNumThreads;
 constexpr int kFp8BlockK = 128;             // e4m3 elements per k-block = one 128 B swizzle row
+// the per-block product needs a second register tile next to the accumulator
+constexpr int kFp8MaxBN = 64, kFp8MaxBNDual = 32;
 
-__host__ __device__ constexpr int p_acc_cols(int BN, bool dual) { return BN * (dual ? 2 : 1); }
-__host__ __device__ constexpr int p_num_acc(int BN, bool dual) { return 2 * p_acc_cols(BN, dual) + 8 * kSfColsPerStage <= 512 ? 2 : 1; }
-__host__ __device__ constexpr uint32_t p_tmem_cols(int BN, bool dual) {
-  int c = p_acc_cols(BN, dual) * p_num_acc(BN, dual) + 8 * kSfColsPerStage;
-  return c <= 32 ? 32 : c <= 64 ? 64 : c <= 128 ? 128 : c <= 256 ? 256 : 512;
-}
 __host__ __device__ constexpr int p_stg_rows(int BN) { return BN < 64 ? BN : 64; }
 __host__ __device__ constexpr int p_staging_bytes(int BN, int out_bytes) { return p_stg_rows(BN) * kTileM * out_bytes; }
 __host__ __device__ constexpr int p_num_stages(int BN, bool dual, int out_bytes) {
-  int s = (225 * 1024 - p_staging_bytes(BN, out_bytes) - 512) / stage_bytes(BN, dual);
+  int s = (225 * 1024 - acc_bytes(BN, dual) - p_staging_bytes(BN, out_bytes) - 512) / stage_bytes(BN, dual);
   return s > 8 ? 8 : s;
 }
 
@@ -96,6 +86,9 @@ __device__ __forceinline__ void fp8_publish_tiles_done(const GemmParams& p, unsi
   }
 }
 
+// ue8m0 -> fp32: 2^(e - 127)
+__device__ __forceinline__ float ue8m0(uint32_t e) { return __uint_as_float(e ? e << 23 : 0x00400000u); }
+
 template <int BN, bool DUAL, typename OutT>
 __global__ void __launch_bounds__(kFp8Threads, 1)
 gemm_fp8_persistent_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_constant__ CUtensorMap tmap_w2,
@@ -103,11 +96,6 @@ gemm_fp8_persistent_kernel(const __grid_constant__ CUtensorMap tmap_w, const __g
                        const int num_tiles) {
   constexpr int STAGES = p_num_stages(BN, DUAL, sizeof(OutT));
   constexpr int STAGE_BYTES = stage_bytes(BN, DUAL);
-  constexpr int ACC_COLS = p_acc_cols(BN, DUAL);
-  constexpr int NUM_ACC = p_num_acc(BN, DUAL);
-  constexpr uint32_t TMEM_COLS = p_tmem_cols(BN, DUAL);
-  constexpr uint32_t IDESC = umma_idesc_mxf8(kTileM, BN);
-  constexpr uint32_t SF_BASE_COL = NUM_ACC * ACC_COLS;   // scale slots sit behind the accumulators
   constexpr int STG_ROWS = p_stg_rows(BN);
   static_assert(STAGES >= 2, "ring too small");
 
@@ -115,45 +103,33 @@ gemm_fp8_persistent_kernel(const __grid_constant__ CUtensorMap tmap_w, const __g
   // 1024 B alignment by *pointer arithmetic* on the __shared__ array: an integer round-trip loses the address space and
   // turns every LDS/STS below into a generic LD.E/ST.E (checked with cuobjdump -sass)
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  OutT* stg = reinterpret_cast<OutT*>(smem + STAGES * STAGE_BYTES);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES + p_staging_bytes(BN, sizeof(OutT)));
+  float* acc_smem = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);   // [BN * (1 + DUAL)][128] fp32
+  OutT* stg = reinterpret_cast<OutT*>(smem + STAGES * STAGE_BYTES + acc_bytes(BN, DUAL));
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES + acc_bytes(BN, DUAL) + p_staging_bytes(BN, sizeof(OutT)));
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tfull_bar = empty_bar + STAGES;   // [2]
-  uint64_t* tempty_bar = tfull_bar + 2;       // [2]
-  uint64_t* sf_full_bar = tempty_bar + 2;     // [STAGES]: scales of the slot are in TMEM
-  uint32_t* tmem_base_smem = reinterpret_cast<uint32_t*>(sf_full_bar + STAGES);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const bool pdl_early = p.expert_offsets != nullptr;
   if (pdl_early) pdl_wait();
 
-  if (warp == 0 && lane == 0) {
+  if (warp == kProducerWarp && lane == 0) {
     tma_prefetch_desc(&tmap_w);
     tma_prefetch_desc(&tmap_x);
     if (DUAL) tma_prefetch_desc(&tmap_w2);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-      mbar_init(&sf_full_bar[s], kSfWarps);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&tfull_bar[a], 1);
-      mbar_init(&tempty_bar[a], kEpiThreads);
+      mbar_init(&empty_bar[s], 4);  // one arrival per MMA warp
     }
     mbar_fence_init();
   }
-  if (warp == 1) tmem_alloc(tmem_base_smem, TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_base_smem;
   // PDL: let the successor's CTAs become resident now (their pre-wait prologue / weight prefetch overlaps this kernel)
   pdl_launch_dependents();
 
   const int kb_total = (p.k + kFp8BlockK - 1) / kFp8BlockK;
 
-  if (warp == 0) {
+  if (warp == kProducerWarp) {
     // ============================================================== TMA producer
     if (elect_one()) {  // one elected lane: uniform-datapath issue, no per-instruction ELECT loop (ptx.cuh)
       // Weights never depend on a predecessor kernel: the first ring-full of weight tiles is requested *before*
@@ -196,99 +172,70 @@ gemm_fp8_persistent_kernel(const __grid_constant__ CUtensorMap tmap_w, const __g
         }
       }
     }
-  } else if (warp == 1) {
-    // ============================================================== MMA issuer
-    if (elect_one()) {  // one elected lane: uniform-datapath issue, no per-instruction ELECT loop (ptx.cuh)
-      uint32_t it = 0, tc = 0;
-      for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-        const TileInfo ti = decode_tile(p, t, tiles_n, tiles_m, BN);
-        if (ti.rows_valid <= 0) continue;
-        const uint32_t ab = tc % NUM_ACC, aph = (tc / NUM_ACC) & 1;
-        mbar_wait(&tempty_bar[ab], aph ^ 1);  // epilogue has drained this accumulator buffer
-        tc_fence_after();
-        const uint32_t acc_addr = tmem_base + ab * ACC_COLS;
-        for (int kb = 0; kb < kb_total; ++kb, ++it) {
-          const uint32_t s = it % STAGES, ph = (it / STAGES) & 1;
-          mbar_wait(&full_bar[s], ph);
-          mbar_wait(&sf_full_bar[s], ph);
-          tc_fence_after();
-          const uint32_t a_addr = smem_u32(smem + s * STAGE_BYTES);
-          const uint32_t b_addr = a_addr + kATileBytes * (DUAL ? 2 : 1);
-          const uint64_t adesc = umma_desc_sw128(a_addr);
-          const uint64_t bdesc = umma_desc_sw128(b_addr);
-          const uint32_t sf = tmem_base + SF_BASE_COL + s * kSfColsPerStage;   // [SFA 4 | SFA2 4 | SFB 8]
-#pragma unroll
-          for (int kk = 0; kk < 4; ++kk) {   // 4 x (K = 32) per 128-element k-block; scale byte kk of the slot's words
-            const uint32_t acc = (kb > 0 || kk > 0) ? 1u : 0u;
-            umma_mxf8(acc_addr, adesc + 2 * kk, bdesc + 2 * kk, umma_idesc_sf(IDESC, kk, kk), sf, sf + 8, acc);
-            if (DUAL) {
-              const uint64_t a2desc = umma_desc_sw128(a_addr + kATileBytes);
-              umma_mxf8(acc_addr + BN, a2desc + 2 * kk, bdesc + 2 * kk, umma_idesc_sf(IDESC, kk, kk), sf + 4, sf + 8, acc);
-            }
-          }
-          umma_commit(&empty_bar[s]);
-        }
-        umma_commit(&tfull_bar[ab]);
-        ++tc;
-      }
-    }
-  } else if (warp >= 6) {
-    // ============================================================== scale staging (4 warps, one per TMEM lane quarter)
-    // Per ring slot: the 32-bit scale words (4 x ue8m0, one per 32-wide K block of this 128-wide k-block) of the stage's 128 weight
-    // rows and BN token rows go to TMEM columns [SFA 4 | SFA2 4 | SFB 8] of the slot: row r -> lane r % 32 (same data in every lane
-    // quarter), column r / 32.  The loads are issued one ring-depth ahead of the MMAs.
-    if (!pdl_early) pdl_wait();   // activation scales are written by the predecessor (quantisation kernel)
-    const uint32_t lane_base = static_cast<uint32_t>((warp & 3) * 32) << 16;
-    const uint32_t grp = static_cast<uint32_t>(warp - 6) >> 2;   // one group alone is bound by its load latency (~0.8 us / slot)
-    uint32_t it = 0;
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-      const TileInfo ti = decode_tile(p, t, tiles_n, tiles_m, BN);
-      if (ti.rows_valid <= 0) continue;
-      for (int kb = 0; kb < kb_total; ++kb, ++it) {
-        if (it % kSfGroups != grp) continue;
-        const uint32_t s = it % STAGES, ph = (it / STAGES) & 1;
-        uint32_t wa[4], wa2[4], wb[8];
-#pragma unroll
-        for (int c = 0; c < 4; ++c) {
-          const size_t r = static_cast<size_t>(ti.w_row + c * 32 + lane);
-          wa[c] = __ldg(p.w_sf + r * p.sf_ld_w + kb);
-          wa2[c] = DUAL ? __ldg(p.w2_sf + r * p.sf_ld_w + kb) : 0u;
-        }
-#pragma unroll
-        for (int c = 0; c < 8; ++c) {
-          const int r = c * 32 + lane;
-          wb[c] = (c * 32 < BN && r < ti.rows_valid) ? __ldcg(p.x_sf + static_cast<size_t>(ti.row_base + r) * p.sf_ld_x + kb) : 0x7f7f7f7fu;
-        }
-        mbar_wait(&empty_bar[s], ph ^ 1);     // the MMAs that read this slot's scales have completed
-        tc_fence_after();
-        const uint32_t sf = tmem_base + lane_base + SF_BASE_COL + s * kSfColsPerStage;
-        tmem_st4(sf, wa);
-        if (DUAL) tmem_st4(sf + 4, wa2);
-        tmem_st8(sf + 8, wb);
-        tmem_st_wait();
-        tc_fence_before();
-        if (elect_one()) mbar_arrive(&sf_full_bar[s]);
-        __syncwarp();
-      }
-    }
   } else {
-    // ============================================================== epilogue warps (128 threads)
-    if (!pdl_early) pdl_wait();  // residual / out are ordered after the predecessor
-    const int q = warp & 3;
-    const int f_local = q * 32 + lane;
-    const int et = threadIdx.x - 64;
+    // ============================================================== MMA warpgroup, then epilogue (128 threads)
+    const int f_local = threadIdx.x;
+    const int et = threadIdx.x;
     constexpr int kVec = 8, kChunks = kTileM / kVec, kRowsPerIter = kEpiThreads / kChunks;
-    uint32_t tc = 0, my_tiles = 0;
+    uint32_t it = 0, tc = 0, my_tiles = 0;
+    if (!pdl_early) pdl_wait();  // activation scales, residual and out are ordered after the predecessor
     for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
       const TileInfo ti = decode_tile(p, t, tiles_n, tiles_m, BN);
       if (ti.rows_valid <= 0) {
         ++my_tiles;  // empty tiles are counted too (EP return: signal_tiles = whole grid)
         continue;
       }
-      const uint32_t ab = tc % NUM_ACC, aph = (tc / NUM_ACC) & 1;
-      mbar_wait(&tfull_bar[ab], aph);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ab * ACC_COLS + (static_cast<uint32_t>(q * 32) << 16);
+      float acc[2][BN / 2], acc2[2][BN / 2];
+      acc_zero<BN>(acc);
+      if (DUAL) acc_zero<BN>(acc2);
+      for (int kb = 0; kb < kb_total; ++kb, ++it) {
+        const uint32_t s = it % STAGES, ph = (it / STAGES) & 1;
+        // scale words (4 x ue8m0, one per 32-wide K block) of this thread's 4 weight rows and BN / 4 token rows
+        uint32_t wa[2][2], wa2[2][2], wb[BN / 4];
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int r = 0; r < 2; ++r) {
+            const size_t row = static_cast<size_t>(ti.w_row + h * 64 + wg_row(2 * r));
+            wa[h][r] = __ldg(p.w_sf + row * p.sf_ld_w + kb);
+            wa2[h][r] = DUAL ? __ldg(p.w2_sf + row * p.sf_ld_w + kb) : 0u;
+          }
+#pragma unroll
+        for (int c = 0; c < BN / 4; ++c) {
+          const int r = wg_col(4 * (c >> 1) + (c & 1));
+          wb[c] = r < ti.rows_valid ? __ldcg(p.x_sf + static_cast<size_t>(ti.row_base + r) * p.sf_ld_x + kb) : 0x7f7f7f7fu;
+        }
+        mbar_wait(&full_bar[s], ph);
+        const uint32_t a_addr = smem_u32(smem + s * STAGE_BYTES);
+        const uint64_t bdesc = gmma_desc_sw128(a_addr + kATileBytes * (DUAL ? 2 : 1));
+#pragma unroll
+        for (int kk = 0; kk < 4; ++kk) {   // 4 x (K = 32) per 128-element k-block; scale byte kk of the words
+          float part[2][BN / 2], part2[2][BN / 2];
+          wgmma_fence();
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            wgmma_e4m3<BN>(part[h], gmma_desc_sw128(a_addr + h * 64 * 128) + 2 * kk, bdesc + 2 * kk);
+            if (DUAL) wgmma_e4m3<BN>(part2[h], gmma_desc_sw128(a_addr + kATileBytes + h * 64 * 128) + 2 * kk, bdesc + 2 * kk);
+          }
+          wgmma_commit();
+          wgmma_wait<0>();
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            wgmma_fence_acc(part[h]);
+            if (DUAL) wgmma_fence_acc(part2[h]);
+#pragma unroll
+            for (int j = 0; j < BN / 2; ++j) {
+              const float sb = ue8m0((wb[2 * (j >> 2) + (j & 1)] >> (8 * kk)) & 0xFF);
+              acc[h][j] += part[h][j] * (ue8m0((wa[h][(j >> 1) & 1] >> (8 * kk)) & 0xFF) * sb);
+              if (DUAL) acc2[h][j] += part2[h][j] * (ue8m0((wa2[h][(j >> 1) & 1] >> (8 * kk)) & 0xFF) * sb);
+            }
+          }
+        }
+        if (lane == 0) mbar_arrive(&empty_bar[s]);
+      }
+      acc_store_smem<BN>(acc, acc_smem, 0);
+      if (DUAL) acc_store_smem<BN>(acc2, acc_smem, BN);
+      named_bar_sync(1, kEpiThreads);
       const int f_glob = ti.n0 + f_local;
       const float bias = (p.bias != nullptr && f_glob < p.n) ? __bfloat162float(p.bias[f_glob]) : 0.0f;
 #pragma unroll 1
@@ -297,17 +244,11 @@ gemm_fp8_persistent_kernel(const __grid_constant__ CUtensorMap tmap_w, const __g
 #pragma unroll 1
         for (int c = c0; c < c0 + STG_ROWS; c += 16) {
           if (c >= ti.rows_valid) break;
-          uint32_t v[16];
           float g[16], u[16];
-          tmem_ld16(taddr + c, v);
-          tmem_ld_wait();
 #pragma unroll
-          for (int j = 0; j < 16; ++j) g[j] = __uint_as_float(v[j]);
-          if (DUAL) {
-            tmem_ld16(taddr + BN + c, v);
-            tmem_ld_wait();
-#pragma unroll
-            for (int j = 0; j < 16; ++j) u[j] = __uint_as_float(v[j]);
+          for (int j = 0; j < 16; ++j) {
+            g[j] = acc_smem[(c + j) * kTileM + f_local];
+            if (DUAL) u[j] = acc_smem[(BN + c + j) * kTileM + f_local];
           }
 #pragma unroll
           for (int j = 0; j < 16; ++j) {
@@ -316,11 +257,6 @@ gemm_fp8_persistent_kernel(const __grid_constant__ CUtensorMap tmap_w, const __g
             if (p.softcap > 0.f) y = p.softcap * tanhf(y / p.softcap);
             stage_store<OutT>(&stg[(c - c0 + j) * kTileM + f_local], y);
           }
-        }
-        if (c0 + STG_ROWS >= ti.rows_valid || c0 + STG_ROWS >= BN) {
-          // last chunk of this tile: the accumulator buffer can be handed back to the MMA warp
-          tc_fence_before();
-          mbar_arrive(&tempty_bar[ab]);
         }
         named_bar_sync(1, kEpiThreads);
         const int ch = et % kChunks;
@@ -362,7 +298,7 @@ gemm_fp8_persistent_kernel(const __grid_constant__ CUtensorMap tmap_w, const __g
             }
           }
         }
-        named_bar_sync(1, kEpiThreads);  // staging buffer free for the next chunk / tile
+        named_bar_sync(1, kEpiThreads);  // staging buffer (and, after the last chunk, the accumulator) free again
       }
       ++my_tiles;
       ++tc;
@@ -373,13 +309,6 @@ gemm_fp8_persistent_kernel(const __grid_constant__ CUtensorMap tmap_w, const __g
       named_bar_sync(1, kEpiThreads);
       if (et == 0) fp8_publish_tiles_done(p, p.signal_peers != nullptr ? my_tiles : tc);
     }
-    tc_fence_before();
-  }
-
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, TMEM_COLS);
   }
 }
 
@@ -392,7 +321,7 @@ int sm_count_cached_fp8() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    if (n <= 0) n = 132;
   }
   return n;
 }
@@ -401,7 +330,7 @@ template <int BN, bool DUAL, typename OutT>
 cudaError_t f_launch_one(const CUtensorMap& tw, const CUtensorMap& tw2, const CUtensorMap& tx, const GemmParams& p, int tiles_n,
                          int tiles_m, int num_tiles, cudaStream_t stream) {
   constexpr int STAGES = p_num_stages(BN, DUAL, sizeof(OutT));
-  constexpr int smem = STAGES * stage_bytes(BN, DUAL) + p_staging_bytes(BN, sizeof(OutT)) + (3 * STAGES + 4) * 8 + 16 + 1024;
+  constexpr int smem = STAGES * stage_bytes(BN, DUAL) + acc_bytes(BN, DUAL) + p_staging_bytes(BN, sizeof(OutT)) + 2 * STAGES * 8 + 1024;
   static_assert(smem <= 227 * 1024, "shared memory budget exceeded");
   auto kern = gemm_fp8_persistent_kernel<BN, DUAL, OutT>;
   static bool configured = false;
@@ -421,9 +350,9 @@ cudaError_t f_dispatch_bn(int bn, const CUtensorMap& tw, const CUtensorMap& tw2,
   switch (bn) {
     case 16: return f_launch_one<16, DUAL, OutT>(tw, tw2, tx, p, tiles_n, tiles_m, num_tiles, s);
     case 32: return f_launch_one<32, DUAL, OutT>(tw, tw2, tx, p, tiles_n, tiles_m, num_tiles, s);
-    case 64: return f_launch_one<64, DUAL, OutT>(tw, tw2, tx, p, tiles_n, tiles_m, num_tiles, s);
-    case 128: return f_launch_one<128, DUAL, OutT>(tw, tw2, tx, p, tiles_n, tiles_m, num_tiles, s);
-    case 256: return f_launch_one<256, DUAL, OutT>(tw, tw2, tx, p, tiles_n, tiles_m, num_tiles, s);
+    case 64:
+      if constexpr (!DUAL) return f_launch_one<64, DUAL, OutT>(tw, tw2, tx, p, tiles_n, tiles_m, num_tiles, s);
+      return cudaErrorInvalidValue;
     default: return cudaErrorInvalidValue;
   }
 }
@@ -433,11 +362,9 @@ cudaError_t f_dispatch_bn(int bn, const CUtensorMap& tw, const CUtensorMap& tw2,
 cudaError_t gemm_fp8_launch(const GemmArgs& a, cudaStream_t stream) {
   const bool dual = a.w2 != nullptr;
   const bool grouped = a.expert_offsets != nullptr;
-  int bn = a.bn > 0 ? a.bn : gemm_pick_bn(a.max_rows);
-  // TMEM budget: accumulators (BN columns, x2 for DUAL) + 128 columns of scale slots must fit the 512 columns of an SM
-  if (dual && bn > 128) bn = 128;
+  const int bn = std::min(a.bn > 0 ? a.bn : gemm_pick_bn(a.max_rows), dual ? kFp8MaxBNDual : kFp8MaxBN);
   if (grouped && (a.n % kTileM) != 0) return cudaErrorInvalidValue;
-  if ((a.k % kFp8BlockK) != 0 || (a.n % kTileM) != 0 || bn > 256) return cudaErrorInvalidValue;   // whole k-blocks / weight tiles only
+  if ((a.k % kFp8BlockK) != 0 || (a.n % kTileM) != 0) return cudaErrorInvalidValue;   // whole k-blocks / weight tiles only
   if (a.w_sf == nullptr || a.x_sf == nullptr || (dual && a.w2_sf == nullptr)) return cudaErrorInvalidValue;
   if (dual && a.out_fp32) return cudaErrorInvalidValue;
 

@@ -1,14 +1,9 @@
-// Persistent variant of the swap-AB tcgen05 GEMM (dense + grouped, no split-K): one CTA per SM walks a static
-// round-robin tile list; the TMA ring never drains between tiles and the TMEM accumulator is double buffered,
-// so tile i's epilogue (TMEM -> registers -> shared -> global) overlaps tile i+1's loads and MMAs.
+// Persistent variant of the swap-AB wgmma GEMM (dense + grouped, no split-K): one CTA per SM walks a static
+// round-robin tile list and the TMA ring never drains between tiles, so tile i+1's weight loads stream while tile i's
+// epilogue runs.  The fixed prologue cost is paid once per SM and everything else is a continuous weight stream.
 //
-// Why: the one-tile-per-CTA kernel (gemm_tcgen05.cu) pays ~5 us of prologue + epilogue per CTA.  For the MoE
-// down-projection of a decode step (1024 tiles of 360 KB) that is ~40% on top of the weight stream — measured
-// 4.65 TB/s vs 6.1 TB/s for the gate/up launch whose tiles are 1 MB (profiles/ncu_gemm_decode.md).  Here the fixed cost is paid
-// once per SM and everything else is a continuous weight stream.
-//
-// Roles (192 threads): warp 0 = TMA producer, warp 1 = MMA issuer (+ TMEM alloc), warps 2..5 = epilogue.
-// Barriers: full/empty per ring stage, tmem_full/tmem_empty per accumulator buffer.
+// Roles (160 threads): warps 0..3 = MMA warpgroup + epilogue, warp 4 = TMA producer.
+// Barriers: full/empty per ring stage.
 #include <algorithm>
 
 #include "gemm_common.cuh"
@@ -21,16 +16,10 @@ using namespace gemm;
 
 namespace {
 
-__host__ __device__ constexpr int p_acc_cols(int BN, bool dual) { return BN * (dual ? 2 : 1); }
-__host__ __device__ constexpr int p_num_acc(int BN, bool dual) { return 2 * p_acc_cols(BN, dual) <= 512 ? 2 : 1; }
-__host__ __device__ constexpr uint32_t p_tmem_cols(int BN, bool dual) {
-  int c = p_acc_cols(BN, dual) * p_num_acc(BN, dual);
-  return c <= 32 ? 32 : c <= 64 ? 64 : c <= 128 ? 128 : c <= 256 ? 256 : 512;
-}
 __host__ __device__ constexpr int p_stg_rows(int BN) { return BN < 64 ? BN : 64; }
 __host__ __device__ constexpr int p_staging_bytes(int BN, int out_bytes) { return p_stg_rows(BN) * kTileM * out_bytes; }
 __host__ __device__ constexpr int p_num_stages(int BN, bool dual, int out_bytes) {
-  int s = (225 * 1024 - p_staging_bytes(BN, out_bytes) - 512) / stage_bytes(BN, dual);
+  int s = (225 * 1024 - acc_bytes(BN, dual) - p_staging_bytes(BN, out_bytes) - 512) / stage_bytes(BN, dual);
   return s > 8 ? 8 : s;
 }
 
@@ -91,10 +80,6 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_
   GemmParams p = p_in;
   constexpr int STAGES = p_num_stages(BN, DUAL, sizeof(OutT));
   constexpr int STAGE_BYTES = stage_bytes(BN, DUAL);
-  constexpr int ACC_COLS = p_acc_cols(BN, DUAL);
-  constexpr int NUM_ACC = p_num_acc(BN, DUAL);
-  constexpr uint32_t TMEM_COLS = p_tmem_cols(BN, DUAL);
-  constexpr uint32_t IDESC = umma_idesc_bf16(kTileM, BN);
   constexpr int STG_ROWS = p_stg_rows(BN);
   static_assert(STAGES >= 2, "ring too small");
 
@@ -102,12 +87,10 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_
   // 1024 B alignment by *pointer arithmetic* on the __shared__ array: an integer round-trip loses the address space and
   // turns every LDS/STS below into a generic LD.E/ST.E (checked with cuobjdump -sass)
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  OutT* stg = reinterpret_cast<OutT*>(smem + STAGES * STAGE_BYTES);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES + p_staging_bytes(BN, sizeof(OutT)));
+  float* acc_smem = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);   // [BN * (1 + DUAL)][128] fp32
+  OutT* stg = reinterpret_cast<OutT*>(smem + STAGES * STAGE_BYTES + acc_bytes(BN, DUAL));
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES + acc_bytes(BN, DUAL) + p_staging_bytes(BN, sizeof(OutT)));
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tfull_bar = empty_bar + STAGES;   // [2]
-  uint64_t* tempty_bar = tfull_bar + 2;       // [2]
-  uint32_t* tmem_base_smem = reinterpret_cast<uint32_t*>(tempty_bar + 2);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -141,31 +124,23 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_
     p.expert_offsets += par * ne;
   }
 
-  if (warp == 0 && lane == 0) {
+  if (warp == kProducerWarp && lane == 0) {
     tma_prefetch_desc(&tmap_w);
     tma_prefetch_desc(&tmap_x);
     if (DUAL) tma_prefetch_desc(&tmap_w2);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&tfull_bar[a], 1);
-      mbar_init(&tempty_bar[a], kEpiThreads);
+      mbar_init(&empty_bar[s], 4);
     }
     mbar_fence_init();
   }
-  if (warp == 1) tmem_alloc(tmem_base_smem, TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_base_smem;
   // PDL: let the successor's CTAs become resident now (their pre-wait prologue / weight prefetch overlaps this kernel)
   pdl_launch_dependents();
 
   const int kb_total = (p.k + kBlockK - 1) / kBlockK;
 
-  if (warp == 0) {
+  if (warp == kProducerWarp) {
     // ============================================================== TMA producer
     if (elect_one()) {  // one elected lane: uniform-datapath issue, no per-instruction ELECT loop (ptx.cuh)
       // Weights never depend on a predecessor kernel: the first ring-full of weight tiles is requested *before*
@@ -208,58 +183,32 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_
         }
       }
     }
-  } else if (warp == 1) {
-    // ============================================================== MMA issuer
-    if (elect_one()) {  // one elected lane: uniform-datapath issue, no per-instruction ELECT loop (ptx.cuh)
-      uint32_t it = 0, tc = 0;
-      for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-        const TileInfo ti = decode_tile(p, t, tiles_n, tiles_m, BN);
-        if (ti.rows_valid <= 0) continue;
-        const uint32_t ab = tc % NUM_ACC, aph = (tc / NUM_ACC) & 1;
-        mbar_wait(&tempty_bar[ab], aph ^ 1);  // epilogue has drained this accumulator buffer
-        tc_fence_after();
-        const uint32_t acc_addr = tmem_base + ab * ACC_COLS;
-        for (int kb = 0; kb < kb_total; ++kb, ++it) {
-          const uint32_t s = it % STAGES, ph = (it / STAGES) & 1;
-          mbar_wait(&full_bar[s], ph);
-          tc_fence_after();
-          const uint32_t a_addr = smem_u32(smem + s * STAGE_BYTES);
-          const uint32_t b_addr = a_addr + kATileBytes * (DUAL ? 2 : 1);
-          const uint64_t adesc = umma_desc_sw128(a_addr);
-          const uint64_t bdesc = umma_desc_sw128(b_addr);
-#pragma unroll
-          for (int kk = 0; kk < kBlockK / kUmmaK; ++kk) {
-            const uint32_t acc = (kb > 0 || kk > 0) ? 1u : 0u;
-            umma_f16(acc_addr, adesc + 2 * kk, bdesc + 2 * kk, IDESC, acc);
-            if (DUAL) {
-              const uint64_t a2desc = umma_desc_sw128(a_addr + kATileBytes);
-              umma_f16(acc_addr + BN, a2desc + 2 * kk, bdesc + 2 * kk, IDESC, acc);
-            }
-          }
-          umma_commit(&empty_bar[s]);
-        }
-        umma_commit(&tfull_bar[ab]);
-        ++tc;
-      }
-    }
   } else {
-    // ============================================================== epilogue warps (128 threads)
-    if (!pdl_early) pdl_wait();  // residual / out are ordered after the predecessor
-    const int q = warp & 3;
-    const int f_local = q * 32 + lane;
-    const int et = threadIdx.x - 64;
+    // ============================================================== MMA warpgroup, then epilogue (128 threads)
+    const int f_local = threadIdx.x;
+    const int et = threadIdx.x;
     constexpr int kVec = 8, kChunks = kTileM / kVec, kRowsPerIter = kEpiThreads / kChunks;
-    uint32_t tc = 0, my_tiles = 0;
+    uint32_t it = 0, tc = 0, my_tiles = 0;
+    bool waited = pdl_early;
     for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
       const TileInfo ti = decode_tile(p, t, tiles_n, tiles_m, BN);
       if (ti.rows_valid <= 0) {
         ++my_tiles;  // empty tiles are counted too (EP return: signal_tiles = whole grid)
         continue;
       }
-      const uint32_t ab = tc % NUM_ACC, aph = (tc / NUM_ACC) & 1;
-      mbar_wait(&tfull_bar[ab], aph);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ab * ACC_COLS + (static_cast<uint32_t>(q * 32) << 16);
+      float acc[2][BN / 2], acc2[2][BN / 2];
+      acc_zero<BN>(acc);
+      if (DUAL) acc_zero<BN>(acc2);
+      mma_mainloop<BN, DUAL, STAGES, STAGE_BYTES, kATileBytes * (DUAL ? 2 : 1)>(
+          acc, acc2, smem, empty_bar, it, kb_total, [&](uint32_t s, uint32_t ph) { mbar_wait(&full_bar[s], ph); });
+      it += kb_total;
+      acc_store_smem<BN>(acc, acc_smem, 0);
+      if (DUAL) acc_store_smem<BN>(acc2, acc_smem, BN);
+      if (!waited) {  // residual / out are ordered after the predecessor
+        pdl_wait();
+        waited = true;
+      }
+      named_bar_sync(1, kEpiThreads);
       const int f_glob = ti.n0 + f_local;
       const float bias = (p.bias != nullptr && f_glob < p.n) ? __bfloat162float(p.bias[f_glob]) : 0.0f;
 #pragma unroll 1
@@ -268,17 +217,11 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_
 #pragma unroll 1
         for (int c = c0; c < c0 + STG_ROWS; c += 16) {
           if (c >= ti.rows_valid) break;
-          uint32_t v[16];
           float g[16], u[16];
-          tmem_ld16(taddr + c, v);
-          tmem_ld_wait();
 #pragma unroll
-          for (int j = 0; j < 16; ++j) g[j] = __uint_as_float(v[j]);
-          if (DUAL) {
-            tmem_ld16(taddr + BN + c, v);
-            tmem_ld_wait();
-#pragma unroll
-            for (int j = 0; j < 16; ++j) u[j] = __uint_as_float(v[j]);
+          for (int j = 0; j < 16; ++j) {
+            g[j] = acc_smem[(c + j) * kTileM + f_local];
+            if (DUAL) u[j] = acc_smem[(BN + c + j) * kTileM + f_local];
           }
 #pragma unroll
           for (int j = 0; j < 16; ++j) {
@@ -287,11 +230,6 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_
             if (p.softcap > 0.f) y = p.softcap * tanhf(y / p.softcap);
             stage_store<OutT>(&stg[(c - c0 + j) * kTileM + f_local], y);
           }
-        }
-        if (c0 + STG_ROWS >= ti.rows_valid || c0 + STG_ROWS >= BN) {
-          // last chunk of this tile: the accumulator buffer can be handed back to the MMA warp
-          tc_fence_before();
-          mbar_arrive(&tempty_bar[ab]);
         }
         named_bar_sync(1, kEpiThreads);
         const int ch = et % kChunks;
@@ -333,24 +271,18 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_
             }
           }
         }
-        named_bar_sync(1, kEpiThreads);  // staging buffer free for the next chunk / tile
+        named_bar_sync(1, kEpiThreads);  // staging buffer (and, after the last chunk, the accumulator) free again
       }
       ++my_tiles;
       ++tc;
     }
+    if (!waited) pdl_wait();
     if (p.signal_flag != nullptr || p.signal_peers != nullptr) {
       // fused stage boundary / EP return: `out` rows went to peer memory; fence once, then report this CTA's tiles
       __threadfence_system();
       named_bar_sync(1, kEpiThreads);
       if (et == 0) publish_tiles_done(p, p.signal_peers != nullptr ? my_tiles : tc);
     }
-    tc_fence_before();
-  }
-
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, TMEM_COLS);
   }
 }
 
@@ -363,7 +295,7 @@ int sm_count_cached() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    if (n <= 0) n = 132;
   }
   return n;
 }
@@ -372,7 +304,7 @@ template <int BN, bool DUAL, typename OutT>
 cudaError_t p_launch_one(const CUtensorMap& tw, const CUtensorMap& tw2, const CUtensorMap& tx, const GemmParams& p, int tiles_n,
                          int tiles_m, int num_tiles, cudaStream_t stream) {
   constexpr int STAGES = p_num_stages(BN, DUAL, sizeof(OutT));
-  constexpr int smem = STAGES * stage_bytes(BN, DUAL) + p_staging_bytes(BN, sizeof(OutT)) + (2 * STAGES + 4) * 8 + 16 + 1024;
+  constexpr int smem = STAGES * stage_bytes(BN, DUAL) + acc_bytes(BN, DUAL) + p_staging_bytes(BN, sizeof(OutT)) + 2 * STAGES * 8 + 1024;
   static_assert(smem <= 227 * 1024, "shared memory budget exceeded");
   auto kern = gemm_persistent_kernel<BN, DUAL, OutT>;
   static bool configured = false;
@@ -393,8 +325,9 @@ cudaError_t p_dispatch_bn(int bn, const CUtensorMap& tw, const CUtensorMap& tw2,
     case 16: return p_launch_one<16, DUAL, OutT>(tw, tw2, tx, p, tiles_n, tiles_m, num_tiles, s);
     case 32: return p_launch_one<32, DUAL, OutT>(tw, tw2, tx, p, tiles_n, tiles_m, num_tiles, s);
     case 64: return p_launch_one<64, DUAL, OutT>(tw, tw2, tx, p, tiles_n, tiles_m, num_tiles, s);
-    case 128: return p_launch_one<128, DUAL, OutT>(tw, tw2, tx, p, tiles_n, tiles_m, num_tiles, s);
-    case 256: return p_launch_one<256, DUAL, OutT>(tw, tw2, tx, p, tiles_n, tiles_m, num_tiles, s);
+    case 128:
+      if constexpr (!DUAL) return p_launch_one<128, DUAL, OutT>(tw, tw2, tx, p, tiles_n, tiles_m, num_tiles, s);
+      return cudaErrorInvalidValue;
     default: return cudaErrorInvalidValue;
   }
 }
@@ -404,7 +337,7 @@ cudaError_t p_dispatch_bn(int bn, const CUtensorMap& tw, const CUtensorMap& tw2,
 cudaError_t gemm_persistent_launch(const GemmArgs& a, cudaStream_t stream) {
   const bool dual = a.w2 != nullptr;
   const bool grouped = a.expert_offsets != nullptr;
-  const int bn = a.bn > 0 ? a.bn : gemm_pick_bn(a.max_rows);
+  const int bn = gemm_clamp_bn(a.bn > 0 ? a.bn : gemm_pick_bn(a.max_rows), dual);
   if (grouped && (a.n % kTileM) != 0) return cudaErrorInvalidValue;
   if ((a.k % 8) != 0 || (a.n % 8) != 0) return cudaErrorInvalidValue;
   if (dual && a.out_fp32) return cudaErrorInvalidValue;

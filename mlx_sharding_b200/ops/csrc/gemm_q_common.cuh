@@ -1,4 +1,4 @@
-// Shared pieces of the quantised (MLX affine int4/int8) tcgen05 GEMMs: the in-register dequantiser and the
+// Shared pieces of the quantised (MLX affine int4/int8) wgmma GEMMs: the in-register dequantiser and the
 // cached TMA descriptor factory for packed codes / transposed scale rows.
 #pragma once
 #include "gemm_common.cuh"

@@ -1,11 +1,11 @@
 // Persistent quantised-weight GEMM (MLX affine int4 / int8, in-kernel dequant) — the production path for 4-bit /
-// 8-bit checkpoints (BASELINE config 2).  Structure = gemm_persistent.cu (static round-robin tile list,
-// double-buffered TMEM accumulator, epilogue overlapped with the next tile) plus a *decoupled* dequant stage:
+// 8-bit checkpoints (BASELINE config 2).  Structure = gemm_persistent.cu (static round-robin tile list, the TMA ring
+// keeps streaming the next tile during the epilogue) plus a *decoupled* dequant stage:
 //
 //   TMA ring (deep, cheap stages)     : packed codes [128 x 32|64 B] + scales/biases rows + bf16 token tile
-//   dequant warps (8, two per row)    : ring stage -> bf16 A tile in a small 128B-swizzled ring (DQ buffers)
-//   MMA warp (1 thread)               : A tile ring + token tile of the ring stage -> TMEM accumulator
-//   epilogue warps (4)                : TMEM -> registers -> shared -> global (shared epilogue semantics)
+//   dequant warps (4, one per row)    : ring stage -> bf16 A tile in a small 128B-swizzled ring (DQ buffers)
+//   MMA warpgroup                     : A tile ring + token tile of the ring stage -> register accumulator, then the
+//                                       epilogue: registers -> shared -> global (shared epilogue semantics)
 //
 // HBM sees 4.5 / 8.5 bits per weight; the deep ring hides HBM latency with ~13-17 KB stages while the expensive
 // 16 KB bf16 tiles only exist DQ (2-3) at a time.
@@ -20,24 +20,18 @@ using namespace gemm;
 
 namespace {
 
-constexpr int kQPThreads = 448;  // warp 0 TMA, 1 MMA, 2..5 epilogue, 6..13 dequant
+constexpr int kQPThreads = kNumThreads + 128;  // warps 0..3 MMA + epilogue, 4 TMA, 5..8 dequant
 
 __host__ __device__ constexpr int qp_packed_bytes(int bits) { return kTileM * (kBlockK * bits / 8); }
 __host__ __device__ constexpr int qp_stage_bytes(int BN, bool dual, int bits) {
   const int d = dual ? 2 : 1;
   return (BN * kBlockK * 2 + (qp_packed_bytes(bits) + 512) * d + 1023) / 1024 * 1024;
 }
-__host__ __device__ constexpr int qp_acc_cols(int BN, bool dual) { return BN * (dual ? 2 : 1); }
-__host__ __device__ constexpr int qp_num_acc(int BN, bool dual) { return 2 * qp_acc_cols(BN, dual) <= 512 ? 2 : 1; }
-__host__ __device__ constexpr uint32_t qp_tmem_cols(int BN, bool dual) {
-  int c = qp_acc_cols(BN, dual) * qp_num_acc(BN, dual);
-  return c <= 32 ? 32 : c <= 64 ? 64 : c <= 128 ? 128 : c <= 256 ? 256 : 512;
-}
-__host__ __device__ constexpr int qp_dq(int BN) { return BN <= 64 ? 3 : 2; }  // bf16 A-tile buffers
+__host__ __device__ constexpr int qp_dq(int BN, bool dual) { return BN <= 64 && !dual ? 3 : 2; }  // bf16 A-tile buffers
 __host__ __device__ constexpr int qp_stg_rows(int BN) { return BN < 64 ? BN : 64; }
 __host__ __device__ constexpr int qp_staging_bytes(int BN, int out_bytes) { return qp_stg_rows(BN) * kTileM * out_bytes; }
 __host__ __device__ constexpr int qp_num_stages(int BN, bool dual, int bits, int out_bytes) {
-  const int fixed = qp_dq(BN) * kATileBytes * (dual ? 2 : 1) + qp_staging_bytes(BN, out_bytes) + 1024;
+  const int fixed = qp_dq(BN, dual) * kATileBytes * (dual ? 2 : 1) + acc_bytes(BN, dual) + qp_staging_bytes(BN, out_bytes) + 1024;
   int s = (225 * 1024 - fixed) / qp_stage_bytes(BN, dual, bits);
   return s > 10 ? 10 : s;
 }
@@ -79,11 +73,7 @@ gemm_q_persistent_kernel(const __grid_constant__ CUtensorMap tmap_wq, const __gr
   constexpr int OFF_PACKED = BN * kBlockK * 2;             // stage layout: [B tile | packed x D | (scales, biases) x D]
   constexpr int OFF_SCALE = OFF_PACKED + PACKED_BYTES * D;
   constexpr uint32_t TX_BYTES = BN * kBlockK * 2 + (PACKED_BYTES + 512) * D;
-  constexpr int DQ = qp_dq(BN);
-  constexpr int ACC_COLS = qp_acc_cols(BN, DUAL);
-  constexpr int NUM_ACC = qp_num_acc(BN, DUAL);
-  constexpr uint32_t TMEM_COLS = qp_tmem_cols(BN, DUAL);
-  constexpr uint32_t IDESC = umma_idesc_bf16(kTileM, BN);
+  constexpr int DQ = qp_dq(BN, DUAL);
   constexpr int STG_ROWS = qp_stg_rows(BN);
   static_assert(STAGES >= 2, "ring too small");
 
@@ -93,50 +83,40 @@ gemm_q_persistent_kernel(const __grid_constant__ CUtensorMap tmap_wq, const __gr
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint8_t* a_ring = smem;                                        // [DQ][D][16 KB]   (1024-aligned)
   uint8_t* ring = a_ring + DQ * D * kATileBytes;                 // [STAGES][STAGE_BYTES]
-  OutT* stg = reinterpret_cast<OutT*>(ring + STAGES * STAGE_BYTES);
+  float* acc_smem = reinterpret_cast<float*>(ring + STAGES * STAGE_BYTES);   // [BN * D][128] fp32
+  OutT* stg = reinterpret_cast<OutT*>(ring + STAGES * STAGE_BYTES + acc_bytes(BN, DUAL));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(reinterpret_cast<uint8_t*>(stg) + qp_staging_bytes(BN, sizeof(OutT)));
   uint64_t* empty_bar = full_bar + STAGES;
   uint64_t* dq_full = empty_bar + STAGES;    // [DQ]
   uint64_t* dq_empty = dq_full + DQ;         // [DQ]
-  uint64_t* tfull_bar = dq_empty + DQ;       // [2]
-  uint64_t* tempty_bar = tfull_bar + 2;      // [2]
-  uint32_t* tmem_base_smem = reinterpret_cast<uint32_t*>(tempty_bar + 2);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
   const bool pdl_early = p.expert_offsets != nullptr;
   if (pdl_early) pdl_wait();
 
-  if (warp == 0 && lane == 0) {
+  if (warp == kProducerWarp && lane == 0) {
     tma_prefetch_desc(&tmap_wq);
     tma_prefetch_desc(&tmap_s);
     tma_prefetch_desc(&tmap_b);
     tma_prefetch_desc(&tmap_x);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], 4);  // one arrival per MMA warp
     }
     for (int j = 0; j < DQ; ++j) {
-      mbar_init(&dq_full[j], 8);   // one arrival per dequant warp
-      mbar_init(&dq_empty[j], 1);  // tcgen05.commit
-    }
-    for (int a = 0; a < 2; ++a) {
-      mbar_init(&tfull_bar[a], 1);
-      mbar_init(&tempty_bar[a], kEpiThreads);
+      mbar_init(&dq_full[j], 4);   // one arrival per dequant warp
+      mbar_init(&dq_empty[j], 4);  // one arrival per MMA warp
     }
     mbar_fence_init();
   }
-  if (warp == 1) tmem_alloc(tmem_base_smem, TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_base_smem;
   if (!pdl_early) pdl_wait();
   pdl_launch_dependents();
 
   const int kb_total = p.k / kBlockK;
 
-  if (warp == 0) {
+  if (warp == kProducerWarp) {
     // ============================================================== TMA producer
     if (elect_one()) {  // one elected lane: uniform-datapath issue, no per-instruction ELECT loop (ptx.cuh)
       uint32_t it = 0;
@@ -161,57 +141,49 @@ gemm_q_persistent_kernel(const __grid_constant__ CUtensorMap tmap_wq, const __gr
         }
       }
     }
-  } else if (warp == 1) {
-    // ============================================================== MMA issuer
-    if (elect_one()) {  // one elected lane: uniform-datapath issue, no per-instruction ELECT loop (ptx.cuh)
-      uint32_t it = 0, tc = 0;
-      for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-        const QTile ti = q_decode_tile(p, t, tiles_n, tiles_m, BN);
-        if (ti.rows_valid <= 0) continue;
-        const uint32_t ab = tc % NUM_ACC, aph = (tc / NUM_ACC) & 1;
-        mbar_wait(&tempty_bar[ab], aph ^ 1);
-        tc_fence_after();
-        const uint32_t acc_addr = tmem_base + ab * ACC_COLS;
-        for (int kb = 0; kb < kb_total; ++kb, ++it) {
-          const uint32_t s = it % STAGES, ph = (it / STAGES) & 1;
-          const uint32_t j = it % DQ, jph = (it / DQ) & 1;
-          mbar_wait(&full_bar[s], ph);   // token tile landed
-          mbar_wait(&dq_full[j], jph);   // weight tile dequantised + fenced
-          tc_fence_after();
-          const uint32_t a_addr = smem_u32(a_ring + j * D * kATileBytes);
-          const uint32_t b_addr = smem_u32(ring + s * STAGE_BYTES);
-          const uint64_t adesc = umma_desc_sw128(a_addr);
-          const uint64_t bdesc = umma_desc_sw128(b_addr);
-#pragma unroll
-          for (int kk = 0; kk < kBlockK / kUmmaK; ++kk) {
-            const uint32_t acc = (kb > 0 || kk > 0) ? 1u : 0u;
-            umma_f16(acc_addr, adesc + 2 * kk, bdesc + 2 * kk, IDESC, acc);
-            if (DUAL) {
-              const uint64_t a2desc = umma_desc_sw128(a_addr + kATileBytes);
-              umma_f16(acc_addr + BN, a2desc + 2 * kk, bdesc + 2 * kk, IDESC, acc);
-            }
-          }
-          umma_commit(&empty_bar[s]);  // ring stage (token tile; packed codes were consumed before dq_full)
-          umma_commit(&dq_empty[j]);   // bf16 A tile buffer
-        }
-        umma_commit(&tfull_bar[ab]);
-        ++tc;
-      }
-    }
-  } else if (warp < 6) {
-    // ============================================================== epilogue warps (128 threads)
-    const int q = warp & 3;
-    const int f_local = q * 32 + lane;
-    const int et = threadIdx.x - 64;
+  } else if (warp < 4) {
+    // ============================================================== MMA warpgroup, then epilogue (128 threads)
+    const int f_local = threadIdx.x;
+    const int et = threadIdx.x;
+    const bool leader = lane == 0;
     constexpr int kVec = 8, kChunks = kTileM / kVec, kRowsPerIter = kEpiThreads / kChunks;
-    uint32_t tc = 0;
+    uint32_t it = 0;
     for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
       const QTile ti = q_decode_tile(p, t, tiles_n, tiles_m, BN);
       if (ti.rows_valid <= 0) continue;
-      const uint32_t ab = tc % NUM_ACC, aph = (tc / NUM_ACC) & 1;
-      mbar_wait(&tfull_bar[ab], aph);
-      tc_fence_after();
-      const uint32_t taddr = tmem_base + ab * ACC_COLS + (static_cast<uint32_t>(q * 32) << 16);
+      float acc[2][BN / 2], acc2[2][BN / 2];
+      acc_zero<BN>(acc);
+      if (DUAL) acc_zero<BN>(acc2);
+      for (int kb = 0; kb < kb_total; ++kb, ++it) {
+        const uint32_t s = it % STAGES, ph = (it / STAGES) & 1;
+        const uint32_t j = it % DQ, jph = (it / DQ) & 1;
+        mbar_wait(&full_bar[s], ph);   // token tile landed
+        mbar_wait(&dq_full[j], jph);   // weight tile dequantised + fenced
+        const uint32_t a_addr = smem_u32(a_ring + j * D * kATileBytes);
+        const uint32_t b_addr = smem_u32(ring + s * STAGE_BYTES);
+        wgmma_fence();
+        mma_kblock<BN>(acc, a_addr, b_addr);
+        if (DUAL) mma_kblock<BN>(acc2, a_addr + kATileBytes, b_addr);
+        wgmma_commit();
+        wgmma_wait<1>();  // the previous k-block's MMAs are done: release its ring stage and A buffer
+        if (kb > 0 && leader) {
+          mbar_arrive(&empty_bar[(it - 1) % STAGES]);
+          mbar_arrive(&dq_empty[(it - 1) % DQ]);
+        }
+      }
+      wgmma_wait<0>();
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        wgmma_fence_acc(acc[h]);
+        if (DUAL) wgmma_fence_acc(acc2[h]);
+      }
+      if (kb_total > 0 && leader) {
+        mbar_arrive(&empty_bar[(it - 1) % STAGES]);
+        mbar_arrive(&dq_empty[(it - 1) % DQ]);
+      }
+      acc_store_smem<BN>(acc, acc_smem, 0);
+      if (DUAL) acc_store_smem<BN>(acc2, acc_smem, BN);
+      named_bar_sync(1, kEpiThreads);
       const int f_glob = ti.n0 + f_local;
       const float bias = (p.bias != nullptr && f_glob < p.n) ? __bfloat162float(p.bias[f_glob]) : 0.0f;
 #pragma unroll 1
@@ -220,17 +192,11 @@ gemm_q_persistent_kernel(const __grid_constant__ CUtensorMap tmap_wq, const __gr
 #pragma unroll 1
         for (int c = c0; c < c0 + STG_ROWS; c += 16) {
           if (c >= ti.rows_valid) break;
-          uint32_t v[16];
           float g[16], u[16];
-          tmem_ld16(taddr + c, v);
-          tmem_ld_wait();
 #pragma unroll
-          for (int j = 0; j < 16; ++j) g[j] = __uint_as_float(v[j]);
-          if (DUAL) {
-            tmem_ld16(taddr + BN + c, v);
-            tmem_ld_wait();
-#pragma unroll
-            for (int j = 0; j < 16; ++j) u[j] = __uint_as_float(v[j]);
+          for (int j = 0; j < 16; ++j) {
+            g[j] = acc_smem[(c + j) * kTileM + f_local];
+            if (DUAL) u[j] = acc_smem[(BN + c + j) * kTileM + f_local];
           }
 #pragma unroll
           for (int j = 0; j < 16; ++j) {
@@ -239,10 +205,6 @@ gemm_q_persistent_kernel(const __grid_constant__ CUtensorMap tmap_wq, const __gr
             if (p.softcap > 0.f) y = p.softcap * tanhf(y / p.softcap);
             stage_store<OutT>(&stg[(c - c0 + j) * kTileM + f_local], y);
           }
-        }
-        if (c0 + STG_ROWS >= ti.rows_valid || c0 + STG_ROWS >= BN) {
-          tc_fence_before();
-          mbar_arrive(&tempty_bar[ab]);
         }
         named_bar_sync(1, kEpiThreads);
         const int ch = et % kChunks;
@@ -296,13 +258,10 @@ gemm_q_persistent_kernel(const __grid_constant__ CUtensorMap tmap_wq, const __gr
           }
         }
       }
-      ++tc;
     }
-    tc_fence_before();
   } else {
-    // ============================================================== dequant producers (8 warps, two threads per row)
-    const int r = (threadIdx.x - 192) & 127;
-    const int half = (threadIdx.x - 192) >> 7;
+    // ============================================================== dequant producers (4 warps, one thread per row)
+    const int r = threadIdx.x - kNumThreads;
     uint32_t it = 0;
     for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
       const QTile ti = q_decode_tile(p, t, tiles_n, tiles_m, BN);
@@ -318,7 +277,9 @@ gemm_q_persistent_kernel(const __grid_constant__ CUtensorMap tmap_wq, const __gr
         for (int d = 0; d < D; ++d) {
           const __nv_bfloat16* sb = reinterpret_cast<const __nv_bfloat16*>(st + OFF_SCALE + d * 512);
           const float sc = __bfloat162float(sb[r]), bi = __bfloat162float(sb[128 + r]);
-          dequant_half_row<BITS>(st + OFF_PACKED + d * PACKED_BYTES + r * (kBlockK * BITS / 8), sc, bi, a_tile + d * kATileBytes, r, half);
+          for (int half = 0; half < 2; ++half)
+            dequant_half_row<BITS>(st + OFF_PACKED + d * PACKED_BYTES + r * (kBlockK * BITS / 8), sc, bi, a_tile + d * kATileBytes, r,
+                                   half);
         }
         fence_proxy_async_smem();
         __syncwarp();
@@ -327,11 +288,6 @@ gemm_q_persistent_kernel(const __grid_constant__ CUtensorMap tmap_wq, const __gr
     }
   }
 
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, TMEM_COLS);
-  }
 }
 
 // ================================================================================================ host side
@@ -343,7 +299,7 @@ int qp_sm_count() {
     int dev = 0;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 148;
+    if (n <= 0) n = 132;
   }
   return n;
 }
@@ -351,8 +307,8 @@ int qp_sm_count() {
 template <int BN, bool DUAL, typename OutT, int BITS>
 cudaError_t qp_launch_one(const QMaps& t, const GemmParams& p, int gk, int tiles_n, int tiles_m, int num_tiles, cudaStream_t stream) {
   constexpr int STAGES = qp_num_stages(BN, DUAL, BITS, sizeof(OutT));
-  constexpr int smem = qp_dq(BN) * kATileBytes * (DUAL ? 2 : 1) + STAGES * qp_stage_bytes(BN, DUAL, BITS) +
-                       qp_staging_bytes(BN, sizeof(OutT)) + (2 * STAGES + 2 * qp_dq(BN) + 4) * 8 + 16 + 1024;
+  constexpr int smem = qp_dq(BN, DUAL) * kATileBytes * (DUAL ? 2 : 1) + STAGES * qp_stage_bytes(BN, DUAL, BITS) + acc_bytes(BN, DUAL) +
+                       qp_staging_bytes(BN, sizeof(OutT)) + (2 * STAGES + 2 * qp_dq(BN, DUAL)) * 8 + 1024;
   static_assert(smem <= 227 * 1024, "shared memory budget exceeded");
   auto kern = gemm_q_persistent_kernel<BN, DUAL, OutT, BITS>;
   static bool configured = false;
@@ -373,8 +329,9 @@ cudaError_t qp_dispatch_bn(int bn, const QMaps& t, const GemmParams& p, int gk, 
     case 16: return qp_launch_one<16, DUAL, OutT, BITS>(t, p, gk, tn, tm, nt, s);
     case 32: return qp_launch_one<32, DUAL, OutT, BITS>(t, p, gk, tn, tm, nt, s);
     case 64: return qp_launch_one<64, DUAL, OutT, BITS>(t, p, gk, tn, tm, nt, s);
-    case 128: return qp_launch_one<128, DUAL, OutT, BITS>(t, p, gk, tn, tm, nt, s);
-    case 256: return qp_launch_one<256, DUAL, OutT, BITS>(t, p, gk, tn, tm, nt, s);
+    case 128:
+      if constexpr (!DUAL) return qp_launch_one<128, DUAL, OutT, BITS>(t, p, gk, tn, tm, nt, s);
+      return cudaErrorInvalidValue;
     default: return cudaErrorInvalidValue;
   }
 }
@@ -391,7 +348,7 @@ cudaError_t qp_dispatch(bool dual, bool fp32, int bn, const QMaps& t, const Gemm
 cudaError_t gemm_q_persistent_launch(const GemmArgs& a, cudaStream_t stream) {
   const bool dual = a.w2 != nullptr;
   const bool grouped = a.expert_offsets != nullptr;
-  const int bn = a.bn > 0 ? a.bn : gemm_pick_bn(a.max_rows);
+  const int bn = gemm_clamp_bn(a.bn > 0 ? a.bn : gemm_pick_bn(a.max_rows), dual);
   if (grouped && (a.n % kTileM) != 0) return cudaErrorInvalidValue;
   if ((a.n % 8) != 0 || (a.k % kBlockK) != 0) return cudaErrorInvalidValue;
   if (dual && a.out_fp32) return cudaErrorInvalidValue;

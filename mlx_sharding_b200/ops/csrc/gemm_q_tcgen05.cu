@@ -1,14 +1,14 @@
-// Quantised-weight variant of the swap-AB tcgen05 GEMM: MLX affine int4 / int8 checkpoints are dequantised
+// Quantised-weight variant of the swap-AB wgmma GEMM: MLX affine int4 / int8 checkpoints are dequantised
 // *inside* the kernel (SURVEY §2.6 K17, §7.4-2 "Plan A").  The reference gets this from MLX's
 // `quantized_matmul` / `gather_qmm` Metal kernels (enabled by `nn.quantize` at shard/utils.py:54-65).
 //
 // Data path per 64-wide k-block (== one or half a quantisation group):
 //   TMA:      packed codes [128 rows x 32|64 B]  + scales[128] + biases[128] (pre-transposed [K/g, rows] at load)
 //             + the bf16 token tile (128B swizzle)                                    -> full barrier
-//   8 dequant warps (two threads per weight row): unpack LSB-first nibbles/bytes, w = s*q + b in fp32, round to bf16,
-//             store into the 128B-swizzled UMMA "A" tile, fence.proxy.async           -> dequant barrier
-//   1 thread: tcgen05.mma (fp32 accumulators in TMEM) ... tcgen05.commit              -> empty barrier
-// so HBM only ever sees 4.5 (or 8.5) bits per weight; everything downstream (TMEM epilogue, DUAL gate/up,
+//   4 dequant warps (one thread per weight row): unpack LSB-first nibbles/bytes, w = s*q + b in fp32, round to bf16,
+//             store into the 128B-swizzled MMA "A" tile, fence.proxy.async            -> dequant barrier
+//   MMA warpgroup: wgmma (fp32 accumulators in registers), wait                        -> empty barrier
+// so HBM only ever sees 4.5 (or 8.5) bits per weight; everything downstream (epilogue, DUAL gate/up,
 // grouped experts, split-K, fused P2P signal) is shared with the dense kernel (gemm_common.cuh).
 #include <mutex>
 #include <unordered_map>
@@ -22,7 +22,7 @@ using namespace gemm;
 
 namespace {
 
-constexpr int kQThreads = 448;  // + warps 6..13: dequant producers (two threads per weight row)
+constexpr int kQThreads = kNumThreads + 128;  // + warps 5..8: dequant producers (one thread per weight row)
 
 __host__ __device__ constexpr int q_stage_bytes(int BN, bool dual, int bits) {
   const int d = dual ? 2 : 1;
@@ -32,7 +32,7 @@ __host__ __device__ constexpr int q_stage_bytes(int BN, bool dual, int bits) {
 __host__ __device__ constexpr int q_num_stages(int BN, bool dual, int bits, int out_bytes) {
   int s = (196 * 1024) / q_stage_bytes(BN, dual, bits);
   s = s > 8 ? 8 : s;
-  while (s * q_stage_bytes(BN, dual, bits) < BN * kTileM * out_bytes) ++s;
+  while (s * q_stage_bytes(BN, dual, bits) < acc_bytes(BN, dual) + BN * kTileM * out_bytes) ++s;
   return s;
 }
 
@@ -52,8 +52,6 @@ gemm_swapab_q_kernel(const __grid_constant__ CUtensorMap tmap_wq, const __grid_c
   constexpr int OFF_PACKED = OFF_B + BN * kBlockK * 2;
   constexpr int OFF_SCALE = OFF_PACKED + PACKED_BYTES * D;  // per weight: scales[128] bf16 then biases[128] bf16
   constexpr uint32_t TX_BYTES = BN * kBlockK * 2 + (PACKED_BYTES + 512) * D;
-  constexpr uint32_t TMEM_COLS = tmem_cols(BN, DUAL);
-  constexpr uint32_t IDESC = umma_idesc_bf16(kTileM, BN);
 
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // 1024 B alignment by *pointer arithmetic* on the __shared__ array: an integer round-trip loses the address space and
@@ -62,15 +60,16 @@ gemm_swapab_q_kernel(const __grid_constant__ CUtensorMap tmap_wq, const __grid_c
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
   uint64_t* deq_bar = full_bar + STAGES;
   uint64_t* empty_bar = deq_bar + STAGES;
-  uint64_t* tmem_full_bar = empty_bar + STAGES;
-  uint32_t* tmem_base_smem = reinterpret_cast<uint32_t*>(tmem_full_bar + 1);
-  uint32_t* flag_smem = tmem_base_smem + 1;
+  uint32_t* flag_smem = reinterpret_cast<uint32_t*>(empty_bar + STAGES);
+  // after the main loop the idle ring holds the fp32 accumulator, then the output staging tile
+  float* acc_smem = reinterpret_cast<float*>(smem);
+  OutT* stg = reinterpret_cast<OutT*>(smem + acc_bytes(BN, DUAL));
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
   // PDL: grouped launches read expert_offsets (written by the permutation kernel) right away, so they wait first;
-  // plain launches overlap their whole prologue (barrier init, TMEM allocation) with the predecessor's tail.
+  // plain launches overlap their whole prologue (barrier init) with the predecessor's tail.
   const bool pdl_early = p.expert_offsets != nullptr;
   if (pdl_early) pdl_wait();
   const int n0 = blockIdx.x * kTileM;
@@ -96,28 +95,23 @@ gemm_swapab_q_kernel(const __grid_constant__ CUtensorMap tmap_wq, const __grid_c
   if (kb_end > kb_total) kb_end = kb_total;
   const int num_kb = kb_end - kb_begin;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == kProducerWarp && lane == 0) {
     tma_prefetch_desc(&tmap_wq);
     tma_prefetch_desc(&tmap_s);
     tma_prefetch_desc(&tmap_b);
     tma_prefetch_desc(&tmap_x);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&deq_bar[s], 8);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&deq_bar[s], 4);
+      mbar_init(&empty_bar[s], 4);
     }
-    mbar_init(tmem_full_bar, 1);
     mbar_fence_init();
   }
-  if (warp == 1) tmem_alloc(tmem_base_smem, TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_base_smem;
   if (!pdl_early) pdl_wait();
   pdl_launch_dependents();
 
-  if (warp == 0) {
+  if (warp == kProducerWarp) {
     // ============================================================== TMA producer
     if (elect_one()) {  // one elected lane: uniform-datapath issue, no per-instruction ELECT loop (ptx.cuh)
       for (int i = 0; i < num_kb; ++i) {
@@ -139,40 +133,23 @@ gemm_swapab_q_kernel(const __grid_constant__ CUtensorMap tmap_wq, const __grid_c
         tma_load_2d(st + OFF_B, &tmap_x, &full_bar[s], kb * kBlockK, row_base, kEvictLast);
       }
     }
-  } else if (warp == 1) {
-    // ============================================================== MMA issuer
-    if (elect_one()) {  // one elected lane: uniform-datapath issue, no per-instruction ELECT loop (ptx.cuh)
-      for (int i = 0; i < num_kb; ++i) {
-        const int s = i % STAGES;
-        const uint32_t ph = (i / STAGES) & 1;
-        mbar_wait(&full_bar[s], ph);  // token tile landed (async proxy)
-        mbar_wait(&deq_bar[s], ph);   // weight tile dequantised + fenced by the producer warps
-        tc_fence_after();
-        const uint32_t a_addr = smem_u32(smem + s * STAGE_BYTES);
-        const uint32_t b_addr = a_addr + OFF_B;
-        const uint64_t adesc = umma_desc_sw128(a_addr);
-        const uint64_t bdesc = umma_desc_sw128(b_addr);
-#pragma unroll
-        for (int kk = 0; kk < kBlockK / kUmmaK; ++kk) {
-          const uint32_t acc = (i > 0 || kk > 0) ? 1u : 0u;
-          umma_f16(tmem_base, adesc + 2 * kk, bdesc + 2 * kk, IDESC, acc);
-          if (DUAL) {
-            const uint64_t a2desc = umma_desc_sw128(a_addr + kATileBytes);
-            umma_f16(tmem_base + BN, a2desc + 2 * kk, bdesc + 2 * kk, IDESC, acc);
-          }
-        }
-        umma_commit(&empty_bar[s]);
-      }
-      umma_commit(tmem_full_bar);
-    }
-  } else if (warp < 6) {
-    // ============================================================== epilogue warps
-    run_epilogue<BN, DUAL, OutT>(p, smem, tmem_base, tmem_full_bar, flag_smem, warp, lane, 64, n0, mt, split, row_base, rows_valid,
-                                 num_kb);
+  } else if (warp < 4) {
+    // ============================================================== MMA warpgroup, then epilogue (128 threads)
+    float acc[2][BN / 2], acc2[2][BN / 2];
+    acc_zero<BN>(acc);
+    if (DUAL) acc_zero<BN>(acc2);
+    mma_mainloop<BN, DUAL, STAGES, STAGE_BYTES, OFF_B>(acc, acc2, smem, empty_bar, 0u, num_kb, [&](uint32_t s, uint32_t ph) {
+      mbar_wait(&full_bar[s], ph);  // token tile landed (async proxy)
+      mbar_wait(&deq_bar[s], ph);   // weight tile dequantised + fenced by the producer warps
+    });
+    named_bar_sync(1, kEpiThreads);  // every warp's MMAs are done: the ring is idle
+    acc_store_smem<BN>(acc, acc_smem, 0);
+    if (DUAL) acc_store_smem<BN>(acc2, acc_smem, BN);
+    named_bar_sync(1, kEpiThreads);
+    run_epilogue<BN, DUAL, OutT>(p, acc_smem, stg, flag_smem, 0, n0, mt, split, row_base, rows_valid);
   } else {
     // ============================================================== dequant producers: one weight row per thread
-    const int r = (threadIdx.x - 192) & 127;   // weight row of the tile
-    const int half = (threadIdx.x - 192) >> 7;  // which 32-weight half of the 64-wide k-block
+    const int r = threadIdx.x - kNumThreads;   // weight row of the tile
     for (int i = 0; i < num_kb; ++i) {
       const int s = i % STAGES;
       const uint32_t ph = (i / STAGES) & 1;
@@ -182,7 +159,9 @@ gemm_swapab_q_kernel(const __grid_constant__ CUtensorMap tmap_wq, const __grid_c
       for (int d = 0; d < D; ++d) {
         const __nv_bfloat16* sb = reinterpret_cast<const __nv_bfloat16*>(st + OFF_SCALE + d * 512);
         const float sc = __bfloat162float(sb[r]), bi = __bfloat162float(sb[128 + r]);
-        dequant_half_row<BITS>(st + OFF_PACKED + d * PACKED_BYTES + r * (kBlockK * BITS / 8), sc, bi, st + d * kATileBytes, r, half);
+        for (int half = 0; half < 2; ++half)
+          dequant_half_row<BITS>(st + OFF_PACKED + d * PACKED_BYTES + r * (kBlockK * BITS / 8), sc, bi, st + d * kATileBytes, r,
+                                 half);
       }
       fence_proxy_async_smem();  // generic-proxy stores -> visible to the tensor core (async proxy)
       __syncwarp();
@@ -190,11 +169,6 @@ gemm_swapab_q_kernel(const __grid_constant__ CUtensorMap tmap_wq, const __grid_c
     }
   }
 
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, TMEM_COLS);
-  }
 }
 
 // ================================================================================================ host side
@@ -257,7 +231,7 @@ bool q_make_tmap(CUtensorMap* m, int kind, const void* ptr, uint64_t d0, uint64_
 template <int BN, bool DUAL, typename OutT, int BITS>
 cudaError_t q_launch_one(const QMaps& t, const GemmParams& p, int group_kblocks, dim3 grid, cudaStream_t stream) {
   constexpr int STAGES = q_num_stages(BN, DUAL, BITS, sizeof(OutT));
-  constexpr int smem = STAGES * q_stage_bytes(BN, DUAL, BITS) + (3 * STAGES + 1) * 8 + 16 + 1024;
+  constexpr int smem = STAGES * q_stage_bytes(BN, DUAL, BITS) + 3 * STAGES * 8 + 16 + 1024;
   static_assert(smem <= 227 * 1024, "shared memory budget exceeded");
   auto kern = gemm_swapab_q_kernel<BN, DUAL, OutT, BITS>;
   static bool configured = false;
@@ -276,8 +250,9 @@ cudaError_t q_dispatch_bn(int bn, const QMaps& t, const GemmParams& p, int gk, d
     case 16: return q_launch_one<16, DUAL, OutT, BITS>(t, p, gk, grid, s);
     case 32: return q_launch_one<32, DUAL, OutT, BITS>(t, p, gk, grid, s);
     case 64: return q_launch_one<64, DUAL, OutT, BITS>(t, p, gk, grid, s);
-    case 128: return q_launch_one<128, DUAL, OutT, BITS>(t, p, gk, grid, s);
-    case 256: return q_launch_one<256, DUAL, OutT, BITS>(t, p, gk, grid, s);
+    case 128:
+      if constexpr (!DUAL) return q_launch_one<128, DUAL, OutT, BITS>(t, p, gk, grid, s);
+      return cudaErrorInvalidValue;
     default: return cudaErrorInvalidValue;
   }
 }
@@ -303,7 +278,7 @@ cudaError_t gemm_q_launch(const GemmArgs& a, cudaStream_t stream) {
   if (!gemm_q_supported(a.q_bits, a.q_group, a.k)) return cudaErrorNotSupported;
   const bool dual = a.w2 != nullptr;
   const bool grouped = a.expert_offsets != nullptr;
-  const int bn = a.bn > 0 ? a.bn : gemm_pick_bn(a.max_rows);
+  const int bn = gemm_clamp_bn(a.bn > 0 ? a.bn : gemm_pick_bn(a.max_rows), dual);
   int splits = a.splits > 0 ? a.splits : 1;
   if (splits == 1 && a.persistent) return gemm_q_persistent_launch(a, stream);
   const int kb_total = a.k / kBlockK;

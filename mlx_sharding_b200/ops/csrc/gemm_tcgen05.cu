@@ -1,18 +1,18 @@
-// Swap-AB tcgen05 GEMM for LLM inference on sm_100a:  Y[tokens, N] = X[tokens, K] · W[N, K]^T
+// Swap-AB wgmma GEMM for LLM inference on sm_90a:  Y[tokens, N] = X[tokens, K] · W[N, K]^T
 //
 // Implements SURVEY §2.6 K3/K4/K5/K8/K9/K11/K12 (all projection GEMMs, the SwiGLU/GeGLU pair, the MoE
 // grouped GEMMs and the LM head) — ops the reference delegates to MLX Metal matmul / gather_qmm
 // (shard/server/model/*.py via mlx_lm blocks).
 //
-// Design (B200-first, not a translation of anything):
-//  * The *weight* tile is the 128-row MMA "A" operand (UMMA_M = 128 output features) and the *token*
-//    tile is the "B" operand (UMMA_N = BN in {16..256} tokens).  Decode batches are skinny (1..64
+// Design:
+//  * The *weight* tile is the MMA "A" operand (128 output features = two wgmma M = 64 halves) and the
+//    *token* tile is the "B" operand (N = BN in {16..128} tokens).  Decode batches are skinny (1..64
 //    tokens) so the tensor-core tile is always full along M and the kernel is a pure HBM weight
-//    stream; prefill uses BN = 256 and gets the same 128x256 tile as a conventional layout.
-//  * TMA (cp.async.bulk.tensor, 128B swizzle) feeds a STAGES-deep shared-memory ring; one elected
-//    thread issues tcgen05.mma with fp32 accumulators in TMEM; 4 epilogue warps read TMEM with
-//    tcgen05.ld, apply the fused epilogue, transpose through shared memory and write coalesced rows.
-//  * DUAL mode streams two weight matrices (gate, up) against the same token tile into two TMEM
+//    stream; prefill uses BN = 128 (64 for the gate/up pair: the accumulators live in registers).
+//  * TMA (cp.async.bulk.tensor, 128B swizzle) feeds a STAGES-deep shared-memory ring; one warpgroup
+//    issues wgmma with fp32 accumulators in registers, then stores them to shared memory, applies the
+//    fused epilogue, transposes through shared memory and writes coalesced rows.
+//  * DUAL mode streams two weight matrices (gate, up) against the same token tile into two register
 //    accumulators and writes act(gate)*up — the SwiGLU intermediate never touches HBM un-fused.
 //  * Grouped mode (MoE): blockIdx.y = expert, rows come from a permuted token buffer via per-expert
 //    offsets; experts with no tokens exit immediately.
@@ -23,6 +23,7 @@
 //    after a system-scope fence — GEMM + P2P hand-off in one kernel, no NCCL call, no host hop.
 #include "gemm_tcgen05.h"
 
+#include <algorithm>
 #include <mutex>
 #include <unordered_map>
 
@@ -40,8 +41,6 @@ gemm_swapab_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_cons
                    const __grid_constant__ CUtensorMap tmap_x, const GemmParams p) {
   constexpr int STAGES = num_stages(BN, DUAL, sizeof(OutT));
   constexpr int STAGE_BYTES = stage_bytes(BN, DUAL);
-  constexpr uint32_t TMEM_COLS = tmem_cols(BN, DUAL);
-  constexpr uint32_t IDESC = umma_idesc_bf16(kTileM, BN);
 
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // 1024B alignment is required by the 128B swizzle atom (8 rows x 128 B)
@@ -50,16 +49,17 @@ gemm_swapab_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_cons
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES);
   uint64_t* empty_bar = full_bar + STAGES;
-  uint64_t* tmem_full_bar = empty_bar + STAGES;
-  uint32_t* tmem_base_smem = reinterpret_cast<uint32_t*>(tmem_full_bar + 1);
-  uint32_t* flag_smem = tmem_base_smem + 1;
+  uint32_t* flag_smem = reinterpret_cast<uint32_t*>(empty_bar + STAGES);
+  // after the main loop the idle ring holds the fp32 accumulator [BN * (1 + DUAL)][128], then the output staging tile
+  float* acc_smem = reinterpret_cast<float*>(smem);
+  OutT* stg = reinterpret_cast<OutT*>(smem + acc_bytes(BN, DUAL));
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
 
   // ---------------------------------------------------------------- tile coordinates
   // PDL: grouped launches read expert_offsets (written by the permutation kernel) right away, so they wait first;
-  // plain launches overlap their whole prologue (barrier init, TMEM allocation) with the predecessor's tail.
+  // plain launches overlap their whole prologue (barrier init) with the predecessor's tail.
   const bool pdl_early = p.expert_offsets != nullptr;
   if (pdl_early) pdl_wait();
   const int n0 = blockIdx.x * kTileM;
@@ -79,7 +79,7 @@ gemm_swapab_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_cons
   }
   rows_valid -= mt * BN;
   row_base += mt * BN;
-  if (rows_valid <= 0) return;  // uniform across the CTA: nothing allocated yet
+  if (rows_valid <= 0) return;  // uniform across the CTA
   if (rows_valid > BN) rows_valid = BN;
   const int w_row = expert * p.n + n0;
 
@@ -91,26 +91,21 @@ gemm_swapab_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_cons
   const int num_kb = kb_end - kb_begin;  // may be 0 for a trailing split: contributes zeros
 
   // ---------------------------------------------------------------- one-time setup
-  if (warp == 0 && lane == 0) {
+  if (warp == kProducerWarp && lane == 0) {
     tma_prefetch_desc(&tmap_w);
     tma_prefetch_desc(&tmap_x);
     if (DUAL) tma_prefetch_desc(&tmap_w2);
     for (int s = 0; s < STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], 4);
     }
-    mbar_init(tmem_full_bar, 1);
     mbar_fence_init();
   }
-  if (warp == 1) tmem_alloc(tmem_base_smem, TMEM_COLS);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_base_smem;
   // PDL: let the successor's CTAs become resident now (their pre-wait prologue / weight prefetch overlaps this kernel)
   pdl_launch_dependents();
 
-  if (warp == 0) {
+  if (warp == kProducerWarp) {
     // ============================================================== TMA producer
     if (elect_one()) {  // one elected lane: uniform-datapath issue, no per-instruction ELECT loop (ptx.cuh)
       // Weights never depend on a predecessor kernel: the first ring-full of weight tiles is requested *before*
@@ -140,55 +135,30 @@ gemm_swapab_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_cons
         tma_load_2d(st + kATileBytes * (DUAL ? 2 : 1), &tmap_x, &full_bar[s], kc, row_base, kEvictLast);
       }
     }
-  } else if (warp == 1) {
-    // ============================================================== MMA issuer (single thread)
-    if (elect_one()) {  // one elected lane: uniform-datapath issue, no per-instruction ELECT loop (ptx.cuh)
-      for (int i = 0; i < num_kb; ++i) {
-        const int s = i % STAGES;
-        const uint32_t ph = (i / STAGES) & 1;
-        mbar_wait(&full_bar[s], ph);
-        tc_fence_after();
-        const uint32_t a_addr = smem_u32(smem + s * STAGE_BYTES);
-        const uint32_t b_addr = a_addr + kATileBytes * (DUAL ? 2 : 1);
-        const uint64_t adesc = umma_desc_sw128(a_addr);
-        const uint64_t bdesc = umma_desc_sw128(b_addr);
-#pragma unroll
-        for (int kk = 0; kk < kBlockK / kUmmaK; ++kk) {
-          const uint32_t acc = (i > 0 || kk > 0) ? 1u : 0u;
-          // advancing 16 bf16 (32 B) along K inside the swizzle atom = +2 in the (addr >> 4) field
-          umma_f16(tmem_base, adesc + 2 * kk, bdesc + 2 * kk, IDESC, acc);
-          if (DUAL) {
-            const uint64_t a2desc = umma_desc_sw128(a_addr + kATileBytes);
-            umma_f16(tmem_base + BN, a2desc + 2 * kk, bdesc + 2 * kk, IDESC, acc);
-          }
-        }
-        umma_commit(&empty_bar[s]);  // frees the smem slot once these MMAs have read it
-      }
-      umma_commit(tmem_full_bar);  // accumulator complete (fires immediately if num_kb == 0)
-    }
   } else {
-    // ============================================================== epilogue warps (128 threads)
+    // ============================================================== MMA warpgroup, then epilogue (128 threads)
+    float acc[2][BN / 2], acc2[2][BN / 2];
+    acc_zero<BN>(acc);
+    if (DUAL) acc_zero<BN>(acc2);
+    mma_mainloop<BN, DUAL, STAGES, STAGE_BYTES, kATileBytes * (DUAL ? 2 : 1)>(
+        acc, acc2, smem, empty_bar, 0u, num_kb, [&](uint32_t s, uint32_t ph) { mbar_wait(&full_bar[s], ph); });
+    named_bar_sync(1, kEpiThreads);  // every warp's MMAs are done: the ring is idle
+    acc_store_smem<BN>(acc, acc_smem, 0);
+    if (DUAL) acc_store_smem<BN>(acc2, acc_smem, BN);
+    named_bar_sync(1, kEpiThreads);
     if (!pdl_early) pdl_wait();  // residual / split-K workspace / out are ordered after the predecessor
-    if (p.cluster_splitk)
-      gemm::cluster_epilogue_store_partial<BN, DUAL>(smem, tmem_base, tmem_full_bar, warp, lane, num_kb);
-    else
-      gemm::run_epilogue<BN, DUAL, OutT>(p, smem, tmem_base, tmem_full_bar, flag_smem, warp, lane, 64, n0, mt, split, row_base,
-                                         rows_valid, num_kb);
+    if (!p.cluster_splitk)
+      gemm::run_epilogue<BN, DUAL, OutT>(p, acc_smem, stg, flag_smem, 0, n0, mt, split, row_base, rows_valid);
   }
   if (p.cluster_splitk) {
-    // split-K through DSMEM: the `splits` CTAs of this output tile are one cluster (gemm_cluster.cuh)
+    // split-K through DSMEM: the `splits` CTAs of this output tile are one cluster (gemm_cluster.cuh); phase A is the
+    // accumulator store above
     __syncwarp();
     gemm::cluster_sync_all();
-    if (warp >= 2) gemm::cluster_epilogue_reduce_store<BN, DUAL, OutT>(p, smem, 64, n0, row_base, rows_valid);
+    if (warp < 4) gemm::cluster_epilogue_reduce_store<BN, DUAL, OutT>(p, smem, 0, n0, row_base, rows_valid);
     __syncwarp();
     gemm::cluster_sync_all();
-    gemm::cluster_signal(p, 64);
-  }
-
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, TMEM_COLS);
+    gemm::cluster_signal(p, 0);
   }
 }
 
@@ -259,7 +229,7 @@ template <int BN, bool DUAL, typename OutT>
 cudaError_t launch_one(const GemmArgs& a, const CUtensorMap& tw, const CUtensorMap& tw2, const CUtensorMap& tx,
                        const GemmParams& p, dim3 grid, cudaStream_t stream) {
   constexpr int STAGES = num_stages(BN, DUAL, sizeof(OutT));
-  constexpr int smem = STAGES * stage_bytes(BN, DUAL) + (2 * STAGES + 1) * 8 + 16 + 1024;
+  constexpr int smem = STAGES * stage_bytes(BN, DUAL) + 2 * STAGES * 8 + 16 + 1024;
   static_assert(smem <= 227 * 1024, "shared memory budget exceeded");
   auto kern = gemm_swapab_kernel<BN, DUAL, OutT>;
   static bool configured = false;
@@ -279,8 +249,9 @@ cudaError_t dispatch_bn(int bn, const GemmArgs& a, const CUtensorMap& tw, const 
     case 16: return launch_one<16, DUAL, OutT>(a, tw, tw2, tx, p, grid, s);
     case 32: return launch_one<32, DUAL, OutT>(a, tw, tw2, tx, p, grid, s);
     case 64: return launch_one<64, DUAL, OutT>(a, tw, tw2, tx, p, grid, s);
-    case 128: return launch_one<128, DUAL, OutT>(a, tw, tw2, tx, p, grid, s);
-    case 256: return launch_one<256, DUAL, OutT>(a, tw, tw2, tx, p, grid, s);
+    case 128:
+      if constexpr (!DUAL) return launch_one<128, DUAL, OutT>(a, tw, tw2, tx, p, grid, s);
+      return cudaErrorInvalidValue;
     default: return cudaErrorInvalidValue;
   }
 }
@@ -315,9 +286,10 @@ int gemm_pick_bn(int max_rows) {
   if (max_rows <= 16) return 16;
   if (max_rows <= 32) return 32;
   if (max_rows <= 64) return 64;
-  if (max_rows <= 128) return 128;
-  return 256;
+  return kMaxBN;
 }
+
+int gemm_clamp_bn(int bn, bool dual) { return std::min(bn, dual ? kMaxBNDual : kMaxBN); }
 
 size_t gemm_workspace_floats(const GemmArgs& a, int bn, int splits) {
   if (splits <= 1) return 0;
@@ -329,7 +301,7 @@ size_t gemm_workspace_floats(const GemmArgs& a, int bn, int splits) {
 cudaError_t gemm_launch(const GemmArgs& a, cudaStream_t stream) {
   const bool dual = a.w2 != nullptr;
   const bool grouped = a.expert_offsets != nullptr;
-  const int bn = a.bn > 0 ? a.bn : gemm_pick_bn(a.max_rows);
+  const int bn = gemm_clamp_bn(a.bn > 0 ? a.bn : gemm_pick_bn(a.max_rows), dual);
   int splits = a.splits > 0 ? a.splits : 1;
   const int kb_total = (a.k + kBlockK - 1) / kBlockK;
   if (splits > kb_total) splits = kb_total;

@@ -1,4 +1,4 @@
-// Host API of the swap-AB tcgen05 GEMM (see gemm_tcgen05.cu).  Plain CUDA, no torch dependency.
+// Host API of the swap-AB wgmma GEMM (see gemm_tcgen05.cu).  Plain CUDA, no torch dependency.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -86,6 +86,7 @@ struct GemmArgs {
 };
 
 int gemm_pick_bn(int max_rows);
+int gemm_clamp_bn(int bn, bool dual);  // largest token tile the register accumulators allow
 size_t gemm_workspace_floats(const GemmArgs& a, int bn, int splits);
 cudaError_t gemm_launch(const GemmArgs& a, cudaStream_t stream);
 cudaError_t gemm_persistent_launch(const GemmArgs& a, cudaStream_t stream);

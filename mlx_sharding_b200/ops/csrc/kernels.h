@@ -1,4 +1,4 @@
-// Host launch API of the non-GEMM sm_100a kernels (plain CUDA; the torch binding lives in bindings.cpp).
+// Host launch API of the non-GEMM sm_90a kernels (plain CUDA; the torch binding lives in bindings.cpp).
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_runtime.h>
@@ -58,7 +58,7 @@ struct FlashPrefillArgs {
 bool flash_prefill_supported(int dk, int dv);
 cudaError_t flash_prefill_launch(const FlashPrefillArgs& a, cudaStream_t s);
 
-// ---- mla_decode.cu (absorbed-latent MLA: tcgen05 decode attention over the cached 576-dim latent, + its prologue)
+// ---- mla_decode.cu (absorbed-latent MLA: wgmma decode attention over the cached 576-dim latent, + its prologue)
 cudaError_t mla_absorbed_prologue_launch(void* q, long long q_ld_t, const void* ckv, long long ckv_ld_t, const void* kpe,
                                          long long pe_ld_t, const void* norm_w, float eps, void* pool, const int* slots,
                                          const int* positions, const float* inv_freq, float mscale, int T, cudaStream_t s);

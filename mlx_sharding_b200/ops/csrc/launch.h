@@ -1,13 +1,13 @@
 // Kernel launch helper with Programmatic Dependent Launch (PDL).
 //
 // A decode step is ~430 small kernels inside one CUDA graph; at that granularity launch latency and each
-// kernel's prologue (barrier init, TMEM allocation, descriptor fetch) are a visible fraction of the step.
+// kernel's prologue (barrier init, descriptor fetch) are a visible fraction of the step.
 // Every kernel in this directory therefore
 //   * is launched with cudaLaunchAttributeProgrammaticStreamSerialization, and
 //   * executes `griddepcontrol.launch_dependents` as early as possible and `griddepcontrol.wait` before it touches any
 //     global memory a predecessor may have written (or writes anything at all),
 // so kernel N+1's blocks are scheduled and run their pre-wait part while kernel N is still running.  For the GEMMs the
-// pre-wait part is barrier init, TMEM allocation *and the first ring-full of weight TMA loads* (weights are never
+// pre-wait part is barrier init *and the first ring-full of weight TMA loads* (weights are never
 // produced by a predecessor), so the HBM latency of a small GEMM hides behind the kernel in front of it.
 // (launch_dependents only takes effect once *every* block of N has issued it, i.e. once all of N's blocks are
 // resident, so the waiting blocks of N+1 can never starve N; completion of N+1 implies completion of N, so N+2's

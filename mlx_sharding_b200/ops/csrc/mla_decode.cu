@@ -1,4 +1,4 @@
-// Absorbed-latent MLA decode attention on tcgen05 / TMEM (SURVEY §2.6 K7, K5 "weight absorption"; VERDICT r1 item 6a).
+// Absorbed-latent MLA decode attention on wgmma (SURVEY §2.6 K7, K5 "weight absorption"; VERDICT r1 item 6a).
 //
 // DeepSeek-V2's MLA caches one 512-dim latent c_t (+ a 64-dim roped key) per token.  The reference decompresses it to 16 heads of
 // K 192 / V 128 and caches *that* (shard/server/model/deepseek_v2.py:120-125 -> 5120 values per token per layer).  With W_UK folded
@@ -11,14 +11,13 @@
 // shared-memory tile, so they run on the tensor cores:
 //
 //   * one CTA per (sequence, KV split); KV tile = one 64-token page = [64 x 576] bf16 fetched by TMA (9 boxes of 64 x 64, 128B
-//     swizzle) into a double-buffered ring;
-//   * S^T[64 tokens, 16 heads] = K_tile[64 x 576] . Q^T: UMMA M=64 (tokens), N=16 (heads), K-major operands, 36 MMAs, fp32 in TMEM;
-//   * the 4 softmax warps read S^T with tcgen05.ld (thread = token row), do the online softmax across the tile with warp shuffles,
-//     write P^T as bf16 into shared memory in the K-major swizzled layout;
+//     swizzle) into a double-buffered ring filled by a producer warp;
+//   * S^T[64 tokens, 16 heads] = K_tile[64 x 576] . Q^T: wgmma M=64 (tokens), N=16 (heads), K-major operands, fp32 in registers;
+//   * the same warpgroup does the online softmax on its S fragment (shuffles within a warp, shared memory across the 4 warps) and
+//     writes P^T as bf16 into shared memory in the K-major swizzled layout;
 //   * O^T[512 dims, 16 heads] = V^T . P^T where V^T is the *same* tile read as an MN-major operand (dims contiguous) — no
-//     transpose, no second copy: 4 UMMA M-tiles of 128 dims x 4 k-steps of 16 tokens;
-//   * S and O accumulators are double-buffered in TMEM, P in shared memory: QK of tile i+1 is issued before PV of tile i, so the
-//     tensor pipe, the softmax warps and the TMA stream overlap; the running O lives in registers (thread = dim row, 64 fp32);
+//     transpose, no second copy: 8 wgmma M-tiles of 64 dims x 4 k-steps of 16 tokens.  The running O stays in the wgmma
+//     accumulator registers (64 fp32 per thread) and is rescaled in place before each PV;
 //   * long contexts are split over CTAs (flash-decoding): partial (o, m, l) in fp32 + a small combine kernel.
 //
 // Decode only (one query token per sequence); prefill chunks take the decompressing path (models/deepseek_v2.py).
@@ -43,27 +42,7 @@ constexpr int kTileBytes = kChunks * kChunkBytes;    // 72 KB
 constexpr int kQChunkBytes = kHeads * 128;           // 2 KB
 constexpr int kQBytes = kChunks * kQChunkBytes;      // 18 KB
 constexpr int kPBytes = kHeads * 128;                // [16 heads x 64 tokens] bf16 = 2 KB
-constexpr int kThreads = 352;                        // warp 0: TMA, warp 1: QK issuer + TMEM, warp 2: PV issuer, warps 3..10: softmax
-constexpr uint32_t kTmemCols = 256;                  // S[2] x 16 + O[2] x 64 = 160 -> 256
-constexpr uint32_t kSCol = 0, kOCol = 32;
-
-constexpr uint32_t idesc(uint32_t M, uint32_t N, uint32_t a_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | (a_mn_major << 15) | ((N >> 3) << 17) | ((M >> 4) << 24);
-}
-constexpr uint32_t kIdescQK = idesc(64, kHeads, 0);
-constexpr uint32_t kIdescPV = idesc(128, kHeads, 1);
-
-// MN-major, 128B-swizzled operand (cute canonical layout ((8,n),(8,k)):((1,LBO),(8,SBO)) in 16-byte units): 64 MN-elements are
-// contiguous (one 128 B line), 8 consecutive K rows are 128 B apart, groups of 8 K rows are SBO apart, 64-element MN blocks LBO apart.
-B200_DEVICE uint64_t umma_desc_mn_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
-  uint64_t d = 0;
-  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
-  d |= static_cast<uint64_t>(lbo_bytes >> 4) << 16;
-  d |= static_cast<uint64_t>(sbo_bytes >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
-  return d;
-}
+constexpr int kThreads = 160;                        // warps 0..3: QK / softmax / PV warpgroup, warp 4: TMA
 
 B200_DEVICE void tma_load_3d(void* smem_dst, const CUtensorMap* m, uint64_t* bar, int c0, int c1, int c2) {
   asm volatile(
@@ -92,30 +71,26 @@ mla_decode_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
   uint8_t* kv_smem = smem;                                   // 2 x 72 KB
   uint8_t* q_smem = smem + 2 * kTileBytes;                   // 18 KB
   uint8_t* p_smem = q_smem + kQBytes;                        // 2 x 2 KB
-  float* red = reinterpret_cast<float*>(p_smem + 2 * kPBytes);   // [2][4][16] cross-warp max / sum
+  float* red = reinterpret_cast<float*>(p_smem + 2 * kPBytes);   // [2][4 warps][16 heads] cross-warp max / sum
   uint64_t* bars = reinterpret_cast<uint64_t*>(red + 2 * 4 * kHeads);
   uint64_t* kv_full = bars;          // [2]
   uint64_t* kv_free = bars + 2;      // [2]
   uint64_t* q_full = bars + 4;
-  uint64_t* s_full = bars + 5;       // [2]
-  uint64_t* p_ready = bars + 7;      // [2]
-  uint64_t* o_full = bars + 9;       // [2]
-  uint32_t* tmem_base_smem = reinterpret_cast<uint32_t*>(bars + 11);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int split = blockIdx.x, b = blockIdx.y;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == 4 && lane == 0) {
     tma_prefetch_desc(&tmap_q);
     tma_prefetch_desc(&tmap_kv);
-    for (int i = 0; i < 11; ++i) mbar_init(&bars[i], 1);
+    for (int i = 0; i < 2; ++i) {
+      mbar_init(&kv_full[i], 1);
+      mbar_init(&kv_free[i], 4);   // one arrival per consumer warp
+    }
+    mbar_init(q_full, 1);
     mbar_fence_init();
   }
-  if (warp == 1) tmem_alloc(tmem_base_smem, kTmemCols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_base_smem;
   pdl_launch_dependents();
   pdl_wait();  // q, the latent pool and the step metadata are written by predecessor kernels
 
@@ -126,7 +101,7 @@ mla_decode_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
   if (t_end > ntiles_seq) t_end = ntiles_seq;
   const int n = t_end > t_begin ? t_end - t_begin : 0;
 
-  if (warp == 0) {
+  if (warp == 4) {
     // ============================================================== TMA producer (whole warp waits, one elected lane issues)
     if (n > 0) {
       if (elect_one()) {
@@ -151,216 +126,157 @@ mla_decode_kernel(const __grid_constant__ CUtensorMap tmap_q, const __grid_const
         __syncwarp();
       }
     }
-  } else if (warp == 1) {
-    // ============================================================== QK issuer (single thread)
-    // The MMAs of this kernel are tiny (64 x 16 x 16: 8 tensor-pipe cycles) while issuing one costs ~50 cycles (descriptor set-up
-    // + the compiler's uniform-datapath election loop), so ONE issuing thread is the bottleneck (measured: 2.1 us per tile).  QK
-    // and PV write different TMEM accumulators and are ordered through mbarriers only, so they get an issuing thread each.
-    if (n > 0) {
-      mbar_wait(q_full, 0);
-      for (int j = 0; j < n; ++j) {
-        const int st = j & 1;
-        mbar_wait(&kv_full[st], (j >> 1) & 1);
-        if (j >= 2) mbar_wait(&p_ready[st], ((j - 2) >> 1) & 1);   // softmax has drained S[st] of tile j-2
-        tc_fence_after();
-        if (elect_one()) {
-          MLA_TRACE(1, j);
-          const uint32_t a0 = smem_u32(kv_smem + st * kTileBytes), b0 = smem_u32(q_smem);
-          const uint32_t d = tmem_base + kSCol + st * kHeads;
+    return;
+  }
+
+  // ============================================================== QK, softmax and PV (one warpgroup)
+  // wgmma fragment (ptx.cuh): element j of an m64n16 accumulator is row wg_row(j), column (head) wg_col(j).  Every thread holds 4
+  // heads, hk(k) = 8 * (k >> 1) + 2 * (lane & 3) + (k & 1) for k = 0..3 (element j belongs to k = 2 * (j >> 2) + (j & 1)), and
+  // two token rows of S.
+  int hk[4];
 #pragma unroll
-          for (int c = 0; c < kChunks; ++c) {
-            const uint64_t ad = umma_desc_sw128(a0 + c * kChunkBytes), bd = umma_desc_sw128(b0 + c * kQChunkBytes);
+  for (int k = 0; k < 4; ++k) hk[k] = 8 * (k >> 1) + 2 * (lane & 3) + (k & 1);
+  float m_run[4], l_run[4], o[8][8];
 #pragma unroll
-            for (int kk = 0; kk < 4; ++kk) umma_f16(d, ad + 2 * kk, bd + 2 * kk, kIdescQK, (c | kk) ? 1u : 0u);
-          }
-          umma_commit(&s_full[st]);
-        }
-        __syncwarp();
-      }
+  for (int k = 0; k < 4; ++k) { m_run[k] = -INFINITY; l_run[k] = 0.f; }
+#pragma unroll
+  for (int m = 0; m < 8; ++m)
+#pragma unroll
+    for (int j = 0; j < 8; ++j) o[m][j] = 0.f;
+  // byte offsets of this thread's P^T elements (K-major 128B-swizzled [16 heads][64 tokens] bf16)
+  uint32_t p_off[8];
+#pragma unroll
+  for (int j = 0; j < 8; ++j) {
+    const int t = wg_row(j), h = wg_col(j);
+    p_off[j] = h * 128 + ((((t >> 3) ^ (h & 7)) & 7) << 4) + (t & 7) * 2;
+  }
+
+  if (n > 0) mbar_wait(q_full, 0);
+  for (int i = 0; i < n; ++i) {
+    const int st = i & 1;
+    mbar_wait(&kv_full[st], (i >> 1) & 1);
+    if (threadIdx.x == 0) MLA_TRACE(1, i);
+    const uint32_t kv0 = smem_u32(kv_smem + st * kTileBytes), q0 = smem_u32(q_smem);
+    float s[8];
+#pragma unroll
+    for (int j = 0; j < 8; ++j) s[j] = 0.f;
+    wgmma_fence();
+#pragma unroll
+    for (int c = 0; c < kChunks; ++c) {
+      const uint64_t ad = gmma_desc_sw128(kv0 + c * kChunkBytes), bd = gmma_desc_sw128(q0 + c * kQChunkBytes);
+#pragma unroll
+      for (int kk = 0; kk < 4; ++kk) wgmma_bf16<16>(s, ad + 2 * kk, bd + 2 * kk);
     }
-  } else if (warp == 2) {
-    // ============================================================== PV issuer (single thread)
-    if (n > 0) {
-      for (int i = 0; i < n; ++i) {
-        const int st = i & 1;
-        mbar_wait(&p_ready[st], (i >> 1) & 1);
-        tc_fence_after();
-        if (elect_one()) {
-          MLA_TRACE(2, i);
-          const uint32_t v0 = smem_u32(kv_smem + st * kTileBytes), p0 = smem_u32(p_smem + st * kPBytes);
-          const uint64_t pd = umma_desc_sw128(p0);
+    wgmma_commit();
+    wgmma_wait<0>();
+    wgmma_fence_acc(s);
+    if (threadIdx.x == 0) MLA_TRACE(3, i);
+
+    bool valid[2];
 #pragma unroll
-          for (int j = 0; j < 4; ++j) {
-            const uint32_t d = tmem_base + kOCol + st * 64 + j * kHeads;
+    for (int r = 0; r < 2; ++r) valid[r] = ((t_begin + i) * kTileTok + wg_row(2 * r)) < ctx;
 #pragma unroll
-            for (int ks = 0; ks < kTileTok / 16; ++ks) {
-              const uint64_t ad = umma_desc_mn_sw128(v0 + (2 * j) * kChunkBytes + ks * 2048, kChunkBytes, 1024);
-              umma_f16(d, ad, pd + 2 * ks, kIdescPV, ks ? 1u : 0u);
-            }
-          }
-          umma_commit(&o_full[st]);
-          // QK(i) finished reading this stage before S(i) was published, so "PV(i) done" frees it
-          umma_commit(&kv_free[st]);
-        }
-        __syncwarp();
-      }
+    for (int j = 0; j < 8; ++j) s[j] = valid[(j >> 1) & 1] ? s[j] * p.scale_log2 : -INFINITY;
+    // tile max per head: the thread's two rows, then the 8 lanes of the warp that hold the same heads, then the 4 warps
+    float tm[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const int j = 4 * (k >> 1) + (k & 1);
+      float v = fmaxf(s[j], s[j + 2]);
+      v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 4));
+      v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 8));
+      v = fmaxf(v, __shfl_xor_sync(0xffffffffu, v, 16));
+      tm[k] = v;
+    }
+    float* rmax = red + (i & 1) * 64;   // [warp][head], double-buffered by tile parity
+    if (lane < 4) {
+#pragma unroll
+      for (int k = 0; k < 4; ++k) rmax[warp * kHeads + hk[k]] = tm[k];
+    }
+    named_bar_sync(1, 128);
+    float alpha[4], mn[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      const float t4 = fmaxf(fmaxf(rmax[hk[k]], rmax[kHeads + hk[k]]), fmaxf(rmax[2 * kHeads + hk[k]], rmax[3 * kHeads + hk[k]]));
+      mn[k] = fmaxf(m_run[k], t4);
+      alpha[k] = (mn[k] == -INFINITY) ? 1.f : exp2f(m_run[k] - mn[k]);
+      m_run[k] = mn[k];
+    }
+    uint8_t* pb = p_smem + st * kPBytes;
+    float psum[4] = {0.f, 0.f, 0.f, 0.f};
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const int k = 2 * (j >> 2) + (j & 1);
+      const float pv = valid[(j >> 1) & 1] ? exp2f(s[j] - mn[k]) : 0.f;   // mn is finite whenever any row of the tile is valid
+      psum[k] += pv;
+      *reinterpret_cast<__nv_bfloat16*>(pb + p_off[j]) = __float2bfloat16_rn(pv);
+    }
+    // the row sum stays thread-private (all threads share m_run, so partial sums add linearly): reduced once at the end
+#pragma unroll
+    for (int k = 0; k < 4; ++k) l_run[k] = l_run[k] * alpha[k] + psum[k];
+    fence_proxy_async_smem();   // generic-proxy P stores -> visible to the tensor core
+    named_bar_sync(1, 128);
+    if (threadIdx.x == 0) MLA_TRACE(4, i);
+
+#pragma unroll
+    for (int m = 0; m < 8; ++m)
+#pragma unroll
+      for (int j = 0; j < 8; ++j) o[m][j] *= alpha[2 * (j >> 2) + (j & 1)];
+    const uint64_t pd = gmma_desc_sw128(smem_u32(pb));
+    wgmma_fence();
+#pragma unroll
+    for (int m = 0; m < 8; ++m)
+#pragma unroll
+      for (int ks = 0; ks < kTileTok / 16; ++ks)
+        wgmma_bf16_ta<16>(o[m], gmma_desc_mn_sw128(kv0 + m * kChunkBytes + ks * 2048, kChunkBytes, 1024), pd + 2 * ks);
+    wgmma_commit();
+    wgmma_wait<0>();
+#pragma unroll
+    for (int m = 0; m < 8; ++m) wgmma_fence_acc(o[m]);
+    if (threadIdx.x == 0) MLA_TRACE(2, i);
+    if (lane == 0) mbar_arrive(&kv_free[st]);   // QK and PV of this tile are done with the stage
+  }
+
+  // ---- row sums: thread-private partials -> CTA totals (once per kernel)
+#pragma unroll
+  for (int k = 0; k < 4; ++k) {
+    float t = l_run[k];
+    t += __shfl_xor_sync(0xffffffffu, t, 4);
+    t += __shfl_xor_sync(0xffffffffu, t, 8);
+    t += __shfl_xor_sync(0xffffffffu, t, 16);
+    l_run[k] = t;
+  }
+  named_bar_sync(1, 128);   // the last tile's maxima have been read
+  if (lane < 4) {
+#pragma unroll
+    for (int k = 0; k < 4; ++k) red[warp * kHeads + hk[k]] = l_run[k];
+  }
+  named_bar_sync(1, 128);
+#pragma unroll
+  for (int k = 0; k < 4; ++k)
+    l_run[k] = (red[hk[k]] + red[kHeads + hk[k]]) + (red[2 * kHeads + hk[k]] + red[3 * kHeads + hk[k]]);
+
+  // ---- write-out: element j of M-tile m is dim 64 * m + wg_row(j) of head wg_col(j)
+  if (p.nsplit == 1) {
+#pragma unroll
+    for (int j = 0; j < 8; ++j) {
+      const int k = 2 * (j >> 2) + (j & 1);
+      const float inv = l_run[k] > 0.f ? 1.0f / l_run[k] : 0.f;
+      __nv_bfloat16* orow = p.out + (size_t)b * p.o_ld_t + (size_t)wg_col(j) * kLat + wg_row(j);
+#pragma unroll
+      for (int m = 0; m < 8; ++m) orow[m * 64] = __float2bfloat16_rn(o[m][j] * inv);
     }
   } else {
-    // ============================================================== softmax + running output (8 warps, 256 threads)
-    // Two warps share each TMEM lane quarter and split the 16 heads (TMEM columns) between them: every thread carries 8 heads,
-    // and each SM sub-partition has two softmax warps to interleave (the per-tile chain is latency-bound with one).
-    constexpr int HH = kHeads / 2;              // heads per thread
-    const int q4 = warp & 3;                    // TMEM lane quarter of this warp
-    const int half = (warp - 3) >> 2;           // 0: heads 0..7, 1: heads 8..15
-    const int h0 = half * HH;
-    const uint32_t lane_addr = static_cast<uint32_t>(q4 * 32) << 16;
-    const int row = q4 * 16 + lane;             // token row of the tile held by this thread (lanes 0..15 only, UMMA M = 64)
-    float m_run[HH], l_run[HH], alpha_prev[HH], o[4 * HH];
+    float* po = p.part_o + ((size_t)b * p.nsplit + split) * kHeads * kLat;
 #pragma unroll
-    for (int h = 0; h < HH; ++h) { m_run[h] = -INFINITY; l_run[h] = 0.f; alpha_prev[h] = 1.f; }
+    for (int j = 0; j < 8; ++j)
 #pragma unroll
-    for (int j = 0; j < 4 * HH; ++j) o[j] = 0.f;
-    // byte offsets of this thread's P^T elements (K-major 128B-swizzled [16 heads][64 tokens] bf16)
-    uint32_t p_off[HH];
+      for (int m = 0; m < 8; ++m) po[(size_t)wg_col(j) * kLat + m * 64 + wg_row(j)] = o[m][j];
+    if (warp == 0 && lane < 4) {   // lanes 0..3 of warp 0 hold all 16 heads between them
+      float* ml = p.part_ml + ((size_t)b * p.nsplit + split) * kHeads * 2;
 #pragma unroll
-    for (int h = 0; h < HH; ++h) {
-      const int hg = h0 + h;
-      p_off[h] = hg * 128 + ((((row >> 3) ^ (hg & 7)) & 7) << 4) + (row & 7) * 2;
+      for (int k = 0; k < 4; ++k) { ml[2 * hk[k]] = m_run[k]; ml[2 * hk[k] + 1] = l_run[k]; }
     }
-
-    auto consume_o = [&](int i) {
-      const int st = i & 1;
-      mbar_wait(&o_full[st], (i >> 1) & 1);
-      tc_fence_after();
-      uint32_t v[4][HH];
-#pragma unroll
-      for (int j = 0; j < 4; ++j) tmem_ld8(tmem_base + lane_addr + kOCol + st * 64 + j * kHeads + h0, v[j]);
-      tmem_ld_wait();
-#pragma unroll
-      for (int j = 0; j < 4; ++j)
-#pragma unroll
-        for (int h = 0; h < HH; ++h) o[j * HH + h] = o[j * HH + h] * alpha_prev[h] + __uint_as_float(v[j][h]);
-      tc_fence_before();
-    };
-
-    for (int i = 0; i < n; ++i) {
-      const int st = i & 1;
-      mbar_wait(&s_full[st], (i >> 1) & 1);
-      if (threadIdx.x == 96) MLA_TRACE(3, i);
-      tc_fence_after();
-      uint32_t v[HH];
-      tmem_ld8(tmem_base + lane_addr + kSCol + st * kHeads + h0, v);
-      tmem_ld_wait();
-      tc_fence_before();
-      const bool valid = lane < 16 && ((t_begin + i) * kTileTok + row) < ctx;
-      float s[HH];
-#pragma unroll
-      for (int h = 0; h < HH; ++h) s[h] = valid ? __uint_as_float(v[h]) * p.scale_log2 : -INFINITY;
-      // tile max per head over the 16 token rows of this warp: transpose-reduce butterfly — after the step with offset `off` a
-      // lane keeps the half of its values selected by that bit of its lane id; lanes 2k, 2k+1 end with the warp max of head k
-      float r4[4], r2[2], r1;
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        const bool up = lane & 8;
-        const float send = up ? s[j] : s[j + 4], keep = up ? s[j + 4] : s[j];
-        r4[j] = fmaxf(keep, __shfl_xor_sync(0xffffffffu, send, 8));
-      }
-#pragma unroll
-      for (int j = 0; j < 2; ++j) {
-        const bool up = lane & 4;
-        const float send = up ? r4[j] : r4[j + 2], keep = up ? r4[j + 2] : r4[j];
-        r2[j] = fmaxf(keep, __shfl_xor_sync(0xffffffffu, send, 4));
-      }
-      {
-        const bool up = lane & 2;
-        const float send = up ? r2[0] : r2[1], keep = up ? r2[1] : r2[0];
-        r1 = fmaxf(keep, __shfl_xor_sync(0xffffffffu, send, 2));
-      }
-      r1 = fmaxf(r1, __shfl_xor_sync(0xffffffffu, r1, 1));
-      // red: [tile parity][half][quarter][8 heads]
-      float* rmax = red + (i & 1) * 64 + half * 32;
-      if (lane < 16 && (lane & 1) == 0) rmax[q4 * HH + (lane >> 1)] = r1;
-      named_bar_sync(1, 256);
-      float alpha[HH];
-#pragma unroll
-      for (int h4 = 0; h4 < HH; h4 += 4) {
-        const float4 a = *reinterpret_cast<const float4*>(rmax + h4), b4 = *reinterpret_cast<const float4*>(rmax + HH + h4);
-        const float4 c4 = *reinterpret_cast<const float4*>(rmax + 2 * HH + h4), d4 = *reinterpret_cast<const float4*>(rmax + 3 * HH + h4);
-        const float tm[4] = {fmaxf(fmaxf(a.x, b4.x), fmaxf(c4.x, d4.x)), fmaxf(fmaxf(a.y, b4.y), fmaxf(c4.y, d4.y)),
-                             fmaxf(fmaxf(a.z, b4.z), fmaxf(c4.z, d4.z)), fmaxf(fmaxf(a.w, b4.w), fmaxf(c4.w, d4.w))};
-#pragma unroll
-        for (int e = 0; e < 4; ++e) {
-          const int h = h4 + e;
-          const float mn = fmaxf(m_run[h], tm[e]);
-          alpha[h] = (mn == -INFINITY) ? 1.f : exp2f(m_run[h] - mn);
-          const float pv = valid ? exp2f(s[h] - mn) : 0.f;   // mn is finite whenever any row of the tile is valid
-          s[h] = pv;
-          // the row sum stays thread-private (all threads share m_run, so partial sums add linearly): reduced once at the end
-          l_run[h] = l_run[h] * alpha[h] + pv;
-          m_run[h] = mn;
-        }
-      }
-      if (lane < 16) {
-        uint8_t* pb = p_smem + st * kPBytes;
-#pragma unroll
-        for (int h = 0; h < HH; ++h) *reinterpret_cast<__nv_bfloat16*>(pb + p_off[h]) = __float2bfloat16_rn(s[h]);
-        fence_proxy_async_smem();
-      }
-      named_bar_sync(1, 256);
-      if (threadIdx.x == 96) { mbar_arrive(&p_ready[st]); MLA_TRACE(4, i); }
-      if (i > 0) consume_o(i - 1);          // overlaps with PV(i) / QK(i+1) on the tensor pipe
-      if (threadIdx.x == 96) MLA_TRACE(5, i);
-#pragma unroll
-      for (int h = 0; h < HH; ++h) alpha_prev[h] = alpha[h];
-    }
-    if (n > 0) consume_o(n - 1);
-
-    // ---- row sums: thread-private partials -> CTA totals (once per kernel)
-    named_bar_sync(1, 256);
-#pragma unroll
-    for (int h = 0; h < HH; ++h) {
-      float t = l_run[h];
-#pragma unroll
-      for (int off = 16; off > 0; off >>= 1) t += __shfl_xor_sync(0xffffffffu, t, off);
-      l_run[h] = t;
-    }
-    float* rsum = red + half * 32;              // [quarter][8 heads]
-    if (lane == 0) {
-#pragma unroll
-      for (int h = 0; h < HH; ++h) rsum[q4 * HH + h] = l_run[h];
-    }
-    named_bar_sync(1, 256);
-#pragma unroll
-    for (int h = 0; h < HH; ++h) l_run[h] = (rsum[h] + rsum[HH + h]) + (rsum[2 * HH + h] + rsum[3 * HH + h]);
-
-    // ---- write-out: thread = dim row (32*q4 + lane) of each of the 4 M-tiles, heads h0..h0+7
-    const int dim0 = q4 * 32 + lane;
-    if (p.nsplit == 1) {
-#pragma unroll
-      for (int h = 0; h < HH; ++h) {
-        const float inv = l_run[h] > 0.f ? 1.0f / l_run[h] : 0.f;
-        __nv_bfloat16* orow = p.out + (size_t)b * p.o_ld_t + (size_t)(h0 + h) * kLat;
-#pragma unroll
-        for (int j = 0; j < 4; ++j) orow[j * 128 + dim0] = __float2bfloat16_rn(o[j * HH + h] * inv);
-      }
-    } else {
-      float* po = p.part_o + ((size_t)b * p.nsplit + split) * kHeads * kLat;
-#pragma unroll
-      for (int h = 0; h < HH; ++h)
-#pragma unroll
-        for (int j = 0; j < 4; ++j) po[(size_t)(h0 + h) * kLat + j * 128 + dim0] = o[j * HH + h];
-      if (q4 == 0 && lane == 0) {               // one thread per head half
-        float* ml = p.part_ml + ((size_t)b * p.nsplit + split) * kHeads * 2;
-#pragma unroll
-        for (int h = 0; h < HH; ++h) { ml[2 * (h0 + h)] = m_run[h]; ml[2 * (h0 + h) + 1] = l_run[h]; }
-      }
-    }
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    tmem_dealloc(tmem_base, kTmemCols);
   }
 }
 
@@ -517,7 +433,7 @@ cudaError_t mla_decode_launch(const void* q, long long q_ld_t, int B, const void
   p.part_o = workspace;
   p.part_ml = workspace != nullptr ? workspace + (size_t)B * nsplit * kHeads * kLat : nullptr;
   if (nsplit > 1 && workspace == nullptr) return cudaErrorInvalidValue;
-  constexpr int smem = 2 * kTileBytes + kQBytes + 2 * kPBytes + 2 * 4 * kHeads * 4 + 12 * 8 + 1024;
+  constexpr int smem = 2 * kTileBytes + kQBytes + 2 * kPBytes + 2 * 4 * kHeads * 4 + 5 * 8 + 1024;
   static_assert(smem <= 227 * 1024, "shared memory budget exceeded");
   static bool configured = false;
   if (!configured) {

@@ -1,9 +1,9 @@
-// Thin inline-PTX wrappers for the sm_100a features used by the kernels in this directory:
-// mbarrier, TMA (cp.async.bulk.tensor), tcgen05 (alloc / mma / commit / ld / fences), and the
-// system-scope release/acquire primitives of the fused P2P stage boundary.
+// Thin inline-PTX wrappers for the sm_90a features used by the kernels in this directory:
+// mbarrier, TMA (cp.async.bulk.tensor), warpgroup MMA (wgmma), and the system-scope release/acquire
+// primitives of the fused P2P stage boundary.
 //
-// Nothing here comes from the reference (it has no native code, SURVEY §2.3); bit layouts follow the
-// PTX ISA as mirrored in cute/arch/mma_sm100_desc.hpp (descriptor unions) of the vendored CUTLASS tree.
+// Nothing here comes from the reference (it has no native code, SURVEY §2.3); descriptor bit layouts follow
+// the PTX ISA ("Matrix Descriptor Format" of the wgmma section).
 #pragma once
 #include <cuda.h>
 #include <cuda_bf16.h>
@@ -18,8 +18,7 @@ B200_DEVICE uint32_t smem_u32(const void* p) { return static_cast<uint32_t>(__cv
 B200_DEVICE uint32_t lane_id() { return threadIdx.x & 31; }
 
 // One elected lane of a fully converged warp.  Unlike `if (lane == 0)`, nvcc knows the branch is warp-uniform-with-one-thread, so
-// tcgen05 / TMA / mbarrier instructions inside it compile to plain uniform-datapath code; under `lane == 0` every such
-// instruction is wrapped in an ELECT / BRA.U.ANY loop with R2UR operand moves (~50 issue cycles per tcgen05.mma, measured).
+// TMA / mbarrier instructions inside it compile to plain uniform-datapath code instead of an ELECT / BRA.U.ANY loop per instruction.
 B200_DEVICE bool elect_one() {
   uint32_t pred;
   asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.u32 %0, 1, 0, p;\n\t}" : "=r"(pred));
@@ -49,7 +48,7 @@ B200_DEVICE bool mbar_try_wait(uint64_t* bar, uint32_t parity) {
       : "memory");
   return ok != 0;
 }
-// Bounded wait: a protocol bug must trap (kernel error), never hang the GPU (gpurun strike policy).
+// Bounded wait: a protocol bug must trap (kernel error), never hang the GPU.
 B200_DEVICE void mbar_wait(uint64_t* bar, uint32_t parity) {
   uint32_t spins = 0;
   while (!mbar_try_wait(bar, parity)) {
@@ -75,101 +74,113 @@ B200_DEVICE void tma_load_2d(void* smem_dst, const CUtensorMap* m, uint64_t* bar
 }
 B200_DEVICE void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
-// ---------------------------------------------------------------------------------------------- tcgen05
-B200_DEVICE void tmem_alloc(uint32_t* smem_out, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_out)), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// ---------------------------------------------------------------------------------------------- wgmma
+// Warpgroup MMA (sm_90a): the four warps of an aligned warpgroup issue together, the fp32 accumulator lives in their registers.
+// Fragment of an m64nN tile: thread t = 32 * w + l holds rows 16 * w + l / 4 + 8 * r and columns 8 * i + 2 * (l % 4) + e in
+// element [4 * i + 2 * r + e] (see wg_row / wg_col).
+B200_DEVICE void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+B200_DEVICE void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+B200_DEVICE void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across the asynchronous MMAs
+template <int N>
+B200_DEVICE void wgmma_fence_acc(float (&d)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-B200_DEVICE void tmem_dealloc(uint32_t taddr, uint32_t ncols) {  // whole warp
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-B200_DEVICE void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-B200_DEVICE void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
+B200_DEVICE int wg_row(int j) { return 16 * ((threadIdx.x >> 5) & 3) + ((threadIdx.x & 31) >> 2) + 8 * ((j >> 1) & 1); }
+B200_DEVICE int wg_col(int j) { return 8 * (j >> 2) + 2 * (threadIdx.x & 3) + (j & 1); }
 
-// D[tmem] (+)= A[smem desc] * B[smem desc]; kind::f16 covers bf16/fp16 inputs with fp32 accumulate
-B200_DEVICE void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// arrive on an mbarrier once all previously issued MMAs of this thread have completed
-B200_DEVICE void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-B200_DEVICE void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// 32 lanes x 16 consecutive fp32 columns: thread i of the warp receives lane (base_lane + i)
-B200_DEVICE void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
-
-// 32 lanes x 8 consecutive fp32 columns
-B200_DEVICE void tmem_ld8(uint32_t taddr, uint32_t (&v)[8]) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0, %1, %2, %3, %4, %5, %6, %7}, [%8];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7])
-      : "r"(taddr)
-      : "memory");
-}
-
-// K-major, 128B-swizzled shared-memory operand descriptor (cute::UMMA::SmemDescriptor):
-//   [0,14) start>>4 | [16,30) LBO>>4 (=1, ignored for swizzled K-major) | [32,46) SBO>>4 (8 rows * 128 B)
-//   [46,48) version=1 (Blackwell) | [61,64) layout type (2 = SWIZZLE_128B)
-B200_DEVICE uint64_t umma_desc_sw128(uint32_t smem_addr) {
+// K-major, 128B-swizzled shared-memory operand descriptor (sm_90 GMMA layout):
+//   [0,14) start>>4 | [16,30) LBO>>4 (=1, ignored for swizzled K-major) | [32,46) SBO>>4 (8 rows * 128 B) | [62,64) 1 = SWIZZLE_128B
+// Advancing 16 bf16 (32 B) along K inside the swizzle atom is +2 in the address field.
+B200_DEVICE uint64_t gmma_desc_sw128(uint32_t smem_addr) {
   uint64_t d = 0;
   d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
   d |= static_cast<uint64_t>(1) << 16;
   d |= static_cast<uint64_t>(1024 >> 4) << 32;
-  d |= static_cast<uint64_t>(1) << 46;
-  d |= static_cast<uint64_t>(2) << 61;
+  d |= static_cast<uint64_t>(1) << 62;
   return d;
 }
-// kind::f16 instruction descriptor (cute::UMMA::InstrDescriptor): fp32 accum, bf16 x bf16, both K-major
-__host__ __device__ constexpr uint32_t umma_idesc_bf16(uint32_t M, uint32_t N) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((N >> 3) << 17) | ((M >> 4) << 24);
+// MN-major, 128B-swizzled operand: 64 MN-elements per 128 B line, 8 K rows 128 B apart, groups of 8 K rows `sbo_bytes` apart,
+// 64-element MN blocks `lbo_bytes` apart.
+B200_DEVICE uint64_t gmma_desc_mn_sw128(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+  uint64_t d = 0;
+  d |= static_cast<uint64_t>((smem_addr & 0x3FFFF) >> 4);
+  d |= static_cast<uint64_t>(lbo_bytes >> 4) << 16;
+  d |= static_cast<uint64_t>(sbo_bytes >> 4) << 32;
+  d |= static_cast<uint64_t>(1) << 62;
+  return d;
 }
 
-// ---- block-scaled FP8 (kind::mxf8f6f4.block_scale): e4m3 x e4m3, fp32 accumulate, one ue8m0 scale per 32 K-elements.
-// Instruction descriptor (cute::UMMA::InstrDescriptorBlockScaled): [4,6) b_sf_id | [7,10) a_format (0 = e4m3) | [10,13) b_format |
-// 15 a_major | 16 b_major | [17,23) N >> 3 | 23 scale format (1 = ue8m0) | [24,29) M >> 4 | [29,31) a_sf_id.
-// a_sf_id / b_sf_id select the byte (0..3) of the 32-bit scale words in TMEM, i.e. which 32-wide K block of the k-block.
-__host__ __device__ constexpr uint32_t umma_idesc_mxf8(uint32_t M, uint32_t N) {
-  return ((N >> 3) << 17) | (1u << 23) | ((M >> 4) << 24);
-}
-__host__ __device__ constexpr uint32_t umma_idesc_sf(uint32_t idesc, uint32_t a_sf_id, uint32_t b_sf_id) {
-  return idesc | (b_sf_id << 4) | (a_sf_id << 29);
-}
-B200_DEVICE void umma_mxf8(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t tmem_sfa, uint32_t tmem_sfb,
-                           uint32_t accumulate) {
+// D (+)= A[smem desc] * B[smem desc], m64nNk16, bf16 inputs, fp32 accumulate; both operands K-major (the _ta form: A MN-major)
+template <int N> B200_DEVICE void wgmma_bf16(float (&d)[N / 2], uint64_t adesc, uint64_t bdesc);
+template <>
+B200_DEVICE void wgmma_bf16<16>(float (&d)[8], uint64_t adesc, uint64_t bdesc) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %6, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::mxf8f6f4.block_scale [%0], %1, %2, %3, [%4], [%5], p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(tmem_sfa), "r"(tmem_sfb), "r"(accumulate)
-      : "memory");
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, 1, 1, 1, 0, 0;"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(adesc), "l"(bdesc));
 }
-// registers -> TMEM: thread i of the warp writes lane (base_lane + i), consecutive 32-bit columns
-B200_DEVICE void tmem_st4(uint32_t taddr, const uint32_t (&v)[4]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x4.b32 [%0], {%1, %2, %3, %4};" ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3])
-               : "memory");
+
+template <>
+B200_DEVICE void wgmma_bf16<32>(float (&d)[16], uint64_t adesc, uint64_t bdesc) {
+  asm volatile(
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, %16, %17, 1, 1, 1, 0, 0;"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "l"(adesc), "l"(bdesc));
 }
-B200_DEVICE void tmem_st8(uint32_t taddr, const uint32_t (&v)[8]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(taddr), "r"(v[0]), "r"(v[1]),
-               "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7])
-               : "memory");
+
+template <>
+B200_DEVICE void wgmma_bf16<64>(float (&d)[32], uint64_t adesc, uint64_t bdesc) {
+  asm volatile(
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, 1, 1, 1, 0, 0;"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(adesc), "l"(bdesc));
 }
-B200_DEVICE void tmem_st_wait() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
+
+// N = 128 as two N = 64 halves: columns 64.. are elements 32.. of the fragment and token rows 64.. of the B tile (+8 KB)
+template <>
+B200_DEVICE void wgmma_bf16<128>(float (&d)[64], uint64_t adesc, uint64_t bdesc) {
+  wgmma_bf16<64>(*reinterpret_cast<float(*)[32]>(&d[0]), adesc, bdesc);
+  wgmma_bf16<64>(*reinterpret_cast<float(*)[32]>(&d[32]), adesc, bdesc + ((64 * 128) >> 4));
+}
+
+template <int N> B200_DEVICE void wgmma_bf16_ta(float (&d)[N / 2], uint64_t adesc, uint64_t bdesc);
+template <>
+B200_DEVICE void wgmma_bf16_ta<16>(float (&d)[8], uint64_t adesc, uint64_t bdesc) {
+  asm volatile(
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, 1, 1, 1, 1, 0;"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(adesc), "l"(bdesc));
+}
+
+template <int N> B200_DEVICE void wgmma_e4m3(float (&d)[N / 2], uint64_t adesc, uint64_t bdesc);  // D = A * B (no accumulate)
+template <>
+B200_DEVICE void wgmma_e4m3<16>(float (&d)[8], uint64_t adesc, uint64_t bdesc) {
+  asm volatile(
+      "wgmma.mma_async.sync.aligned.m64n16k32.f32.e4m3.e4m3 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7}, %8, %9, 0, 1, 1;"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "l"(adesc), "l"(bdesc));
+}
+
+template <>
+B200_DEVICE void wgmma_e4m3<32>(float (&d)[16], uint64_t adesc, uint64_t bdesc) {   // two N = 16 halves (see wgmma_bf16<128>)
+  wgmma_e4m3<16>(*reinterpret_cast<float(*)[8]>(&d[0]), adesc, bdesc);
+  wgmma_e4m3<16>(*reinterpret_cast<float(*)[8]>(&d[8]), adesc, bdesc + ((16 * 128) >> 4));
+}
+
+template <>
+B200_DEVICE void wgmma_e4m3<64>(float (&d)[32], uint64_t adesc, uint64_t bdesc) {   // two N = 32 halves (see wgmma_bf16<128>)
+  wgmma_e4m3<32>(*reinterpret_cast<float(*)[16]>(&d[0]), adesc, bdesc);
+  wgmma_e4m3<32>(*reinterpret_cast<float(*)[16]>(&d[16]), adesc, bdesc + ((32 * 128) >> 4));
+}
+
 
 // ---------------------------------------------------------------------------------------------- scopes
 B200_DEVICE void st_release_sys(uint32_t* p, uint32_t v) {
@@ -202,7 +213,7 @@ B200_DEVICE void named_bar_sync(uint32_t id, uint32_t nthreads) {
 B200_DEVICE void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 B200_DEVICE void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 // Small kernels: release the successor first (its CTAs become resident and run their pre-wait prologue — for the GEMMs that is
-// barrier init, TMEM alloc and the first ring-full of *weight* TMA loads), then wait for the predecessor.  Nothing before the
+// barrier init and the first ring-full of *weight* TMA loads), then wait for the predecessor.  Nothing before the
 // wait may touch memory a predecessor writes; completion of grid i+1 implies completion of grid i, so the chain stays ordered.
 B200_DEVICE void pdl_sync() { pdl_launch_dependents(); pdl_wait(); }
 

@@ -2,7 +2,7 @@
 
 Three roles:
   1. the CPU execution path (tests, gloo plumbing config, machines without a GPU);
-  2. the numerical oracle every sm_100a kernel in ``ops/csrc`` is tested against;
+  2. the numerical oracle every sm_90a kernel in ``ops/csrc`` is tested against;
   3. on CUDA tensors it *is* the "straight PyTorch + cuBLAS" same-box baseline (``baseline/``).
 
 Each function documents which upstream behaviour (SURVEY §2.2 U1–U12, §2.6 K1–K17) it reproduces.
@@ -22,7 +22,7 @@ NAME = "reference"
 
 # Oracle mode (default): every matmul accumulates and returns true fp32.  ``FAST_BASELINE = True`` turns
 # this module into the "straight PyTorch + cuBLAS" baseline: bf16 tensor-core GEMMs via F.linear with bf16
-# outputs, the way a plain PyTorch re-implementation of the reference pipeline would run on a B200.
+# outputs, the way a plain PyTorch re-implementation of the reference pipeline would run on an H100.
 FAST_BASELINE = False
 
 

@@ -1,4 +1,4 @@
-"""Weight containers shared by the PyTorch oracle and the sm_100a kernels.
+"""Weight containers shared by the PyTorch oracle and the sm_90a kernels.
 
 ``LinearWeight`` holds either a dense ``[N, K]`` matrix (row = output feature, K contiguous — the
 K-major layout TMA/UMMA want) or the MLX affine-quantised triple (SURVEY U10).  A leading expert

@@ -113,6 +113,7 @@ class DecodeLoop:
         m.boundary = None
         if self.last:
             toks, _, _, _ = O.sample(out, self.temps, self.top_p, None, 0)
+            self._toks[g] = toks
             if self.transport == "fused":
                 self.p2p.send_tokens(toks, g)
             else:
@@ -170,6 +171,7 @@ class DecodeLoop:
         """Capture one graph per group.  NCCL transport keeps send/recv outside the graph."""
         self._steps_done = [0] * self.G
         self._outs = [None] * self.G
+        self._toks = [None] * self.G   # last stage: the tokens each group's step sampled
         if not self.use_graphs:
             return
         from ..ops import b200 as _b
@@ -220,7 +222,7 @@ class DecodeLoop:
                 self.groups[g].graph.replay()
                 out = self._outs[g]
             else:
-                out = self._body(g)
+                out = self._outs[g] = self._body(g)
             self._nccl_post(g, out)
             self._steps_done[g] += 1
 

@@ -136,7 +136,7 @@ class ExpertParallelMoE:
         offs, total, x_perm, row_dst = C.ep_regroup(
             b.base + b.off_recv_count, st[W + 2:W + 3].data_ptr(), st[-1:].data_ptr(),
             b.base + b.off_recv_meta, b.base + b.off_recv_x, W, b.cap, self.E_local, b.H, b.dev, min(W * b.cap, W * Tmax * k), b.t_ret_y)
-        # 3) my experts: grouped swap-AB tcgen05 GEMMs on the received rows; the down-projection epilogue stores every output
+        # 3) my experts: grouped swap-AB wgmma GEMMs on the received rows; the down-projection epilogue stores every output
         #    row straight into its source rank's return buffer (peer memory) and the last tile bumps all sources' flags
         max_rows = min(W * Tmax, x_perm.shape[0])  # upper bound of rows one expert can receive (every rank sends <= Tmax)
         exp_rows = T * k  # balanced routing: a rank receives about as many pairs as it sends (only picks the token tile size)

@@ -6,7 +6,7 @@ allocated with ``cudaMalloc`` and exported through CUDA IPC.  After the handle e
 (``torch.distributed`` object all-gather on the control group) stage ``i`` holds a device pointer into
 stage ``i+1``'s inbox, and the last stage one into stage 0's token inbox.
 
-Hand-off = the *last kernel of the stage* (the down-proj tcgen05 GEMM epilogue for dense layers, the
+Hand-off = the *last kernel of the stage* (the down-proj wgmma GEMM epilogue for dense layers, the
 MoE weighted-combine for DeepSeek MoE layers) stores its output rows straight into the peer inbox and
 the last CTA bumps the peer's flag with a system-scope release (``models/base.py::_final_kwargs``,
 ``csrc/gemm_tcgen05.cu``, ``csrc/moe.cu``).  The consumer's step begins with a one-thread

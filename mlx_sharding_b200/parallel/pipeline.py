@@ -15,7 +15,7 @@ ids) that stage 0 builds and every stage copies host->device from pinned memory.
 control plane      ``ShmControl`` (default, one node): launch ring in shared memory — publishing a step is a memcpy, picking
                    it up is a poll; no pickle, no gloo, no system call per step.  ``DistControl``: gloo broadcast fallback for
                    ranks that do not share a host.
-data plane         ``FusedPlane`` (B200, default): resident inboxes mapped over CUDA IPC; the *last kernel of a stage* (down-proj
+data plane         ``FusedPlane`` (CUDA, default): resident inboxes mapped over CUDA IPC; the *last kernel of a stage* (down-proj
                    GEMM epilogue / MoE combine) stores its rows straight into the next stage's inbox over NVLink and bumps its
                    flag; the consumer's step starts with a flag-wait kernel.  A decode step of a group is ONE CUDA-graph replay
                    per stage: no NCCL call, no host hop, no control message on the hand-off.  ``DistPlane``: ``send/recv`` over
@@ -417,7 +417,7 @@ def build_chain(stage: StageExecutor, num_groups: Optional[int] = None, max_toke
                 transport: str = "auto", control: str = "auto"):
     """Collective over all ranks: set up the control plane and the data plane of a chain.  Returns ``(ctl, plane)``.
 
-    transport: ``fused`` (B200 kernels + CUDA IPC inboxes), ``nccl`` / ``gloo`` (two-sided), ``auto`` = fused on CUDA with the
+    transport: ``fused`` (native kernels + CUDA IPC inboxes), ``nccl`` / ``gloo`` (two-sided), ``auto`` = fused on CUDA with the
     b200 backend when every rank is on this host, else nccl on CUDA, gloo on CPU.
     control: ``shm`` / ``dist`` / ``auto`` (shm when every rank is on this host)."""
     import socket

@@ -3,8 +3,7 @@
 The reference serves HTTP from the process that runs the model (``shard/openai_api.py:487-517``: one ``HTTPServer``, the handler owns
 the generation loop).  With continuous batching that design puts every stream's per-token work — incremental detokenisation, the
 JSON chunk, the socket write — on threads that share the interpreter lock with the engine loop: at a few hundred streams the
-handlers hold the lock most of the time, the engine thread queues behind them, and the GPUs idle (measured on 4 x B200,
-Llama-3-8B: 1.4 k tokens/s over HTTP against 42 k through the same engine without HTTP).
+handlers hold the lock most of the time, the engine thread queues behind them, and the GPUs idle.
 
 ``--api-workers N`` moves the front end out:
 

@@ -581,7 +581,7 @@ def run(host: str, port: int, model_provider: ModelProvider, static_dir: str, ap
 
 
 def build_arg_parser() -> argparse.ArgumentParser:
-    p = argparse.ArgumentParser(description="B200-native OpenAI-compatible HTTP server (mlx-sharding-api).")
+    p = argparse.ArgumentParser(description="H100-native OpenAI-compatible HTTP server (mlx-sharding-api).")
     p.add_argument("--model", type=str, help="The path to the model weights, tokenizer, and config")
     p.add_argument("--adapter-path", type=str, help="Optional path for trained adapter weights (accepted, unused)")
     p.add_argument("--host", type=str, default="127.0.0.1", help="Host for the HTTP server (default: 127.0.0.1)")
@@ -607,7 +607,7 @@ def build_arg_parser() -> argparse.ArgumentParser:
     p.add_argument("--max-prefill-tokens", type=int, default=2048, help="prompt tokens per prefill step (chunked prefill)")
     p.add_argument("--transport", type=str, default="auto", choices=["auto", "fused", "nccl", "gloo"],
                    help="stage hand-off of the native chain (torchrun): fused = GEMM-epilogue P2P store over NVLink (default on "
-                        "B200), nccl / gloo = send/recv")
+                        "CUDA), nccl / gloo = send/recv")
     p.add_argument("--prefix-cache", action="store_true",
                    help="automatic prefix caching: full KV pages of prompt prefixes are shared between requests (chat system "
                         "prompts are prefilled once); not available with gRPC reference shards")

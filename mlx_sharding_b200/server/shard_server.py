@@ -63,7 +63,7 @@ def serve_chain(model_path: str, start_layer=None, end_layer=None, device=None, 
 
 
 def main(argv=None):
-    parser = argparse.ArgumentParser(description="Pipeline-stage server (B200-native mlx-sharding-server)")
+    parser = argparse.ArgumentParser(description="Pipeline-stage server (H100-native mlx-sharding-server)")
     parser.add_argument("--model", type=str, required=True, help="Path to the model or HF repo")
     parser.add_argument("-s", "--start-layer", type=int, default=None, help="Start layer index for model sharding")
     parser.add_argument("-e", "--end-layer", type=int, default=None, help="End layer index for model sharding")

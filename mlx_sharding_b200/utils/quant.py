@@ -7,7 +7,7 @@ Format (SURVEY U10; consumed by the reference through ``nn.quantize`` at shard/u
 * ``biases``  : ``fp16|bf16[out, in / group_size]``
 * ``w[o, i] = scales[o, i // g] * q[o, i] + biases[o, i // g]``
 
-These helpers are the CPU oracle for the in-kernel dequantisation done by the sm_100a GEMM /
+These helpers are the CPU oracle for the in-kernel dequantisation done by the sm_90a GEMM /
 embedding kernels (``ops/csrc``) and are used by the synthetic-checkpoint generator.
 """
 from __future__ import annotations
@@ -110,7 +110,7 @@ def repack_int4_pairs(wq: torch.Tensor) -> torch.Tensor:
 def to_mxfp8(w: torch.Tensor):
     """``w [..., K]`` (any float dtype, ``K % 32 == 0``) -> ``(q uint8 [..., K], sf uint8 [..., K / 32])``: e4m3 elements with one
     shared power-of-two scale (ue8m0, ``2^(sf - 127)``) per 32 consecutive ``K`` values, ``scale = 2^ceil(log2(amax / 448))``.
-    The load-time format of weights for ``ops/csrc/gemm_fp8.cu`` (``tcgen05.mma kind::mxf8f6f4.block_scale``); the activation side
+    The load-time format of weights for ``ops/csrc/gemm_fp8.cu`` (wgmma e4m3 with per-32 block scales); the activation side
     is produced by ``elementwise.cu::quant_mxfp8_kernel`` with the same rule, bit for bit."""
     K = w.shape[-1]
     assert K % 32 == 0

@@ -1,7 +1,7 @@
 """Measurement helpers: CUDA-event timing (max over ranks), clock / throttle sampling, L2 flush.
 
 The reference's only instrumentation is a wall-clock tokens-per-second print (generate.py:114-122,
-SURVEY §5.1); these follow the B200 profiling recipe instead: device-timed, warm-up first, clocks sampled
+SURVEY §5.1); these follow a GPU profiling recipe instead: device-timed, warm-up first, clocks sampled
 *during* the timed region, multi-GPU numbers reported as the max over ranks.
 """
 from __future__ import annotations
@@ -99,7 +99,7 @@ _flush_buf = None
 
 
 def flush_l2(nbytes: int = 256 << 20):
-    """Write a buffer larger than the 126 MB L2 so the next kernel starts cold."""
+    """Write a buffer larger than the 50 MB L2 so the next kernel starts cold."""
     global _flush_buf
     if _flush_buf is None or _flush_buf.numel() < nbytes:
         _flush_buf = torch.empty(nbytes, dtype=torch.uint8, device="cuda")

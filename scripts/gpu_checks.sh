@@ -1,5 +1,5 @@
 #!/bin/bash
-# The GPU validation commands used for profiles/ (run from the repo root on a B200 box; under gpurun: `gpurun -- 'bash scripts/gpu_checks.sh tests'`).
+# GPU validation commands (run from the repo root on an H100 box):
 #   bash scripts/gpu_checks.sh tests            # 1 GPU: kernel + model tests, smoke
 #   bash scripts/gpu_checks.sh tests-mgpu       # >= 2 GPUs: pipeline / expert-parallel parity
 #   bash scripts/gpu_checks.sh bench N          # headline bench on N GPUs (N > 1: both shardings)

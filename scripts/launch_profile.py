@@ -49,7 +49,7 @@ def summarise(path, out, title):
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--summarise", nargs=2)
-    ap.add_argument("--title", default="Launch list of one decode step (DeepSeek-Coder-V2-Lite bf16, 1xB200, 64 sequences, context 128)")
+    ap.add_argument("--title", default="Launch list of one decode step (DeepSeek-Coder-V2-Lite bf16, 1 GPU, 64 sequences, context 128)")
     ap.add_argument("--batch", type=int, default=64)
     ap.add_argument("--ctx", type=int, default=128)
     a = ap.parse_args()

@@ -45,7 +45,7 @@ def main():
     hdr_lines = [f"# ncu --set full: every kernel launched by `__graft_entry__.smoke()` ({len(data)} launches, {len(seen)} distinct kernels)", "",
           "`ncu --set full --clock-control none --import-source on -c 200` under `gpurun` (1 GPU) over the smoke decode of the tiny DeepSeek-V2 flagship",
           "(prefill + graph-free decode steps through `LLMEngine`).  One row per distinct kernel = its first captured launch; the tiny model makes every",
-          "kernel latency-bound, so read this table as *coverage* (each hand-written kernel ran on the B200 and was captured with source) — the",
+          "kernel latency-bound, so read this table as *coverage* (each hand-written kernel ran and was captured with source) — the",
           "roofline-relevant captures are `ncu_decode_kernels.md` and `ncu_gemm_persistent.md`.  Durations under ncu are not benchmark numbers.", ""]
     if title is not None:
         hdr_lines = [f"# {title} ({len(data)} launches, {len(seen)} distinct kernels)", "",

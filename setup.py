@@ -6,7 +6,7 @@ from setuptools import find_packages, setup
 setup(
     name="mlx-sharding-b200",
     version="0.1.0",
-    description="Blackwell-native pipeline-parallel LLM inference engine with the capabilities of mlx_sharding",
+    description="Hopper-native pipeline-parallel LLM inference engine with the capabilities of mlx_sharding",
     packages=find_packages(include=["mlx_sharding_b200", "mlx_sharding_b200.*", "shard", "shard.*"]),
     py_modules=["generate", "sharding_weight"],
     python_requires=">=3.10",

@@ -1,5 +1,5 @@
 // Split-K / tile sweep for the decode-shaped GEMMs: device time per launch measured by replaying a CUDA graph
-// of launches that rotate over enough weight copies to defeat the 126 MB L2 (weights are streamed from HBM,
+// of launches that rotate over enough weight copies to defeat the 50 MB L2 (weights are streamed from HBM,
 // as in a real decode step).  Prints one line per (shape, splits).
 #include <cstdio>
 #include <cstdlib>

@@ -1,5 +1,5 @@
-// Standalone correctness + timing harness for the tcgen05 GEMM (no torch): compares against a naive
-// fp32 CUDA reference on the shapes the models use.  Build: see tests/cuda/build.sh; run on the B200 box.
+// Standalone correctness + timing harness for the wgmma GEMM (no torch): compares against a naive
+// fp32 CUDA reference on the shapes the models use.  Build: see tests/cuda/build.sh; run on an H100.
 #include <cstdio>
 #include <cstdlib>
 #include <cmath>

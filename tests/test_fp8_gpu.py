@@ -1,4 +1,4 @@
-"""Block-scaled FP8 (MXFP8) on sm_100a: the activation quantiser, the tcgen05 kind::mxf8f6f4.block_scale GEMM (dense, DUAL,
+"""Block-scaled FP8 (MXFP8) on sm_90a: the activation quantiser, the wgmma e4m3 GEMM with per-32 block scales (dense, DUAL,
 grouped with offsets, grouped scatter layout) against fp32 matmuls of the *same* MXFP8 operands, and the error budget of
 FP8 expert banks against the bf16 / MLX-affine oracle."""
 import pytest
@@ -103,4 +103,4 @@ def test_fp8_expert_bank_error_budget(monkeypatch):
         monkeypatch.setenv("MLXB200_FP8_EXPERTS", "1")
         got = b200.moe_block(xx, gw, rk, *mk(), "silu")
         rel = ((got.float() - ref.float()).norm() / ref.float().norm()).item()
-        assert rel < 0.09, rel     # e4m3 operands on both sides, two chained GEMMs: ~6.5 % of the block output norm (docs/FP8.md)
+        assert rel < 0.09, rel     # e4m3 operands on both sides, two chained GEMMs: ~6.5 % of the block output norm

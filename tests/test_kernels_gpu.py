@@ -1,4 +1,4 @@
-"""GPU numerics: every sm_100a kernel vs the plain-PyTorch fp32 reference of the same op (SURVEY §4)."""
+"""GPU numerics: every sm_90a kernel vs the plain-PyTorch fp32 reference of the same op (SURVEY §4)."""
 import math
 
 import pytest
@@ -318,7 +318,7 @@ def _qweight(*shape, bits=4, group=64, seed=0):
 @pytest.mark.parametrize("bits,group", [(4, 64), (8, 64), (4, 128)])
 @pytest.mark.parametrize("T", [1, 64, 300])
 def test_quantized_linear_in_kernel_dequant(B, bits, group, T):
-    """int4/int8 MLX-affine weights dequantised inside the tcgen05 GEMM == dequantise-then-matmul oracle."""
+    """int4/int8 MLX-affine weights dequantised inside the wgmma GEMM == dequantise-then-matmul oracle."""
     K, N = 2048, 1408
     x = rnd(T, K)
     W = _qweight(N, K, bits=bits, group=group, seed=1)

@@ -1,4 +1,4 @@
-"""Absorbed-latent MLA on sm_100a (ops/csrc/mla_decode.cu): the tcgen05 multi-query decode kernel over the cached 576-dim latent,
+"""Absorbed-latent MLA on sm_90a (ops/csrc/mla_decode.cu): the wgmma multi-query decode kernel over the cached 576-dim latent,
 its fused prologue, and the whole DeepSeek stage on the folded weights — each against a plain PyTorch fp32 reference."""
 import math
 
@@ -100,7 +100,7 @@ MLA_CFG = dict(model_type="deepseek_v2", vocab_size=512, hidden_size=512, interm
 
 
 def test_stage_on_absorbed_weights_matches_decompressed_cache():
-    """Whole DeepSeek stage: latent cache + folded weights + tcgen05 latent attention (decode) / decompressing prefill (chunked, so
+    """Whole DeepSeek stage: latent cache + folded weights + wgmma latent attention (decode) / decompressing prefill (chunked, so
     the second chunk attends to cached latents) vs the default decompressed K/V cache — same weights, bf16 tolerances."""
     from helpers import run_sequence
     from mlx_sharding_b200.models.deepseek_v2 import DeepseekV2Stage

@@ -1,4 +1,4 @@
-"""GPU end-to-end: stage models on the b200 (sm_100a kernels) backend vs the PyTorch reference backend
+"""GPU end-to-end: stage models on the b200 (sm_90a kernels) backend vs the PyTorch reference backend
 with identical bf16 weights — logits agree, greedy tokens agree, engine runs batched requests."""
 import pytest
 import torch
