@@ -28,14 +28,13 @@ _EXPERT_RE = re.compile(r"^(model\.layers\.\d+\.mlp)\.experts\.(\d+)\.(gate_proj
 
 class DeepseekV2Stage(StageModel):
     arch = "deepseek_v2"
-    overlap_shared_experts = os.environ.get("MLXB200_OVERLAP_SHARED", "1") != "0"
     # KV layout: cache the 512-dim latent + the 64-dim roped key (one shared "head", 576 values per token) instead of the
     # reference's decompressed per-head K/V (16 x (192 + 128) = 5120 values, shard/server/model/deepseek_v2.py:120-125) and absorb
     # kv_b into the query / output side.  Mathematically identical attention (see ``_attn_absorbed``).
     #   None (default): automatic — on when the sm_90a latent-attention kernel supports the shapes (16 heads, kv_lora_rank 512,
     #                   rope 64, no q-LoRA, unquantised attention weights, 64-token pages: DeepSeek-V2-Lite / Coder-V2-Lite);
-    #   MLXB200_ABSORBED_MLA=0 / 1 forces it off / on (``1`` on the reference backend selects the einsum formulation).
-    absorbed_mla = {"0": False, "1": True}.get(os.environ.get("MLXB200_ABSORBED_MLA", ""), None)
+    #   a subclass may set True (on the reference backend that selects the einsum formulation ``_attn_absorbed``).
+    absorbed_mla = None
 
     def __init__(self, cfg, spec=None, dtype=torch.bfloat16, device="cpu", backend=None):
         super().__init__(cfg, spec, dtype, device, backend)
@@ -81,8 +80,6 @@ class DeepseekV2Stage(StageModel):
             raise NotImplementedError("absorbed-latent MLA kernel: 16 heads, kv_lora_rank 512, rope 64, no q-LoRA (DeepSeek-V2-Lite shapes)")
         if any(w[k].is_quantized for w in self.layer_weights.values() for k in ("qkv_a", "kv_b", "o") if k in w):
             # quantised attention weights keep their packed form (and the reference's cache layout): folding would expand them
-            if os.environ.get("MLXB200_ABSORBED_MLA") == "1":
-                raise NotImplementedError("absorbed-latent MLA with quantised attention weights")
             self.absorbed_mla = False
             return
         nh, nope, rd, vd, lr, H = c.num_attention_heads, c.qk_nope_head_dim, c.qk_rope_head_dim, c.v_head_dim, c.kv_lora_rank, c.hidden_size
@@ -163,14 +160,6 @@ class DeepseekV2Stage(StageModel):
             # decode step on the absorbed weights: one GEMM -> [q_abs | q_pe] x 16 heads, c_kv, k_pe; fused prologue (latent norm,
             # both ropes, cache append); wgmma multi-query attention over the cached latent; folded output projection
             qkv = O.linear(normed, w["qkv_abs"])
-            if self.backend_name == "b200" and "router" in w and w.get("e_gate") is not None and not w["e_gate"].is_quantized \
-                    and not O.fp8_experts_enabled(w["e_gate"]):
-                nb = O.l2_prefetch_bytes()
-                if nb > 0 and T <= 128:
-                    # forked AFTER the q/kv projection (the chain's bandwidth-hungry kernel): HBM mostly idles from here to the
-                    # expert GEMMs.  Pull the first experts of this layer's gate / up banks into L2 on the side stream (the grouped
-                    # GEMM walks the experts in order, so these are the tiles of its first waves)
-                    O.prefetch_aside([O._dense(w["e_gate"]), O._dense(w["e_up"])], nb)
             qa = qkv[:, : nh * (lr + rd)].unflatten(1, (nh, lr + rd))
             O.mla_absorbed_prologue(qa, qkv[:, nh * (lr + rd): nh * (lr + rd) + lr], qkv[:, nh * (lr + rd) + lr:], w["kv_a_ln"],
                                     c.rms_norm_eps, kpool, meta, self.rope)
@@ -219,8 +208,6 @@ class DeepseekV2Stage(StageModel):
         o_lat = O.paged_attention(torch.cat([q_abs, q[..., nope:]], -1), kpool, vpool, meta, c.attn_scale, 0.0)   # [T, nh, lr]
         return torch.einsum("thl,hvl->thv", o_lat.float(), wkv[:, nope:]).to(q.dtype).reshape(T, nh * vd)
 
-    fuse_shared = os.environ.get("MLXB200_FUSE_SHARED", "1") != "0"
-
     def _convert_quantized_for_b200(self):
         """Load-time policy for MLX 4/8-bit checkpoints on the CUDA backend (BASELINE config 2; off with MLXB200_FP8_EXPERTS=0, which
         keeps every weight packed and dequantised in-kernel with exact MLX-affine semantics):
@@ -247,7 +234,7 @@ class DeepseekV2Stage(StageModel):
                     w[k] = LinearWeight(weight=w[k].dense(self.dtype).contiguous(), bias=w[k].bias)
             if "router" not in w or w.get("e_gate") is None or H % 128 or I % 128:
                 continue
-            fuse = bool(ns and self.fuse_shared and "s_gate" in w and w["s_gate"].out_features == ns * I)
+            fuse = bool(ns and "s_gate" in w and w["s_gate"].out_features == ns * I)
 
             def bank(ek, sk, down=False):
                 parts = [w[ek].dense(torch.bfloat16)]
@@ -273,7 +260,7 @@ class DeepseekV2Stage(StageModel):
         35 MB of weights) disappear into the persistent grouped GEMMs that already stream the bank at the HBM roofline; the router
         kernel emits the extra (id, 1.0) columns itself."""
         c = self.cfg
-        if not (self.fuse_shared and self.backend_name == "b200" and self.expert_shard is None and c.n_shared_experts):
+        if not (self.backend_name == "b200" and self.expert_shard is None and c.n_shared_experts):
             return
         ns, I, H = c.n_shared_experts, c.moe_intermediate_size, c.hidden_size
         for w in self.layer_weights.values():
@@ -312,7 +299,7 @@ class DeepseekV2Stage(StageModel):
         nh, nope, rd, vd, lr = c.num_attention_heads, c.qk_nope_head_dim, c.qk_rope_head_dim, c.v_head_dim, c.kv_lora_rank
         page = kpool.shape[2]
         lat = O.rmsnorm(ckv, w["kv_a_ln"], c.rms_norm_eps)                                      # [T, lr]
-        if getattr(meta, "fresh", False) and self.rope.interleaved and os.environ.get("MLXB200_PREFILL_FAST", "1") != "0":
+        if getattr(meta, "fresh", False) and self.rope.interleaved:
             # Fresh prompts (no cached context; the TTFT case): everything the batch attends to is this chunk itself, so the
             # per-head K / V come straight from the chunk's own latents — no gather of cached pages, no concatenate / transpose
             # passes.  kv_b on the T rows, then ONE fused launch ropes q_pe in place and writes K = [k_nope | rope(k_pe)] and V
@@ -357,8 +344,10 @@ class DeepseekV2Stage(StageModel):
     def mlp_block(self, i, h, meta: BatchMeta):
         O, c, w = self.ops, self.cfg, self.layer_weights[i]
         T = h.shape[0]
-        ep = getattr(self, "ep_layers", None)
-        if "router" in w and "s_gate" not in w and hasattr(O, "moe_block") and not (ep is not None and i in ep):
+        ep = getattr(self, "ep_layers", {}).get(i)   # this layer's expert-parallel block (parallel/ep.py), if any
+        rk = dict(top_k=c.num_experts_per_tok, method=c.topk_method, n_group=c.n_group or 1, topk_group=c.topk_group or 1,
+                  scaling=c.routed_scaling_factor, norm_topk=c.norm_topk_prob)
+        if "router" in w and "s_gate" not in w and hasattr(O, "moe_block") and ep is None:
             # CUDA backend, whole bank local, shared experts riding in the bank: the block is router -> grouped gate-up -> grouped
             # down -> combine, with BOTH RMSNorms around it folded in — the pre-MoE norm into the router kernel and the next layer's
             # input norm into the combine (decode batches; ops/b200.py::moe_block falls back to separate norm kernels otherwise)
@@ -366,16 +355,13 @@ class DeepseekV2Stage(StageModel):
             fk = self._final_kwargs(i, T, "mlp")
             nxt = self.layer_weights.get(i + 1) if not fk else None
             nn = dict(next_norm=(nxt["in_ln"], c.rms_norm_eps)) if (nxt is not None and "in_ln" in nxt and self.spec.runs_attn(i + 1)) else {}
-            res = O.moe_block(h, w["router"], dict(top_k=c.num_experts_per_tok, method=c.topk_method, n_group=c.n_group or 1,
-                                                   topk_group=c.topk_group or 1, scaling=c.routed_scaling_factor,
-                                                   norm_topk=c.norm_topk_prob),
-                              w["e_gate"], w["e_up"], w["e_down"], "silu", residual=h, pre_norm=(w["post_ln"], c.rms_norm_eps),
-                              **extra, **nn, **fk)
+            res = O.moe_block(h, w["router"], rk, w["e_gate"], w["e_up"], w["e_down"], "silu", residual=h,
+                              pre_norm=(w["post_ln"], c.rms_norm_eps), **extra, **nn, **fk)
             if nn:
                 self._prenormed = res
                 return res[0]
             return res
-        if ("router" in w and ep is not None and i in ep and hasattr(ep[i], "route_forward") and getattr(ep[i].b, "v2", False)
+        if ("router" in w and ep is not None and hasattr(ep, "route_forward") and getattr(ep.b, "v2", False)
                 and 1 <= T <= 1024 and os.environ.get("MLXB200_EP_FUSED_ROUTE", "1") != "0"):
             # expert-parallel block as four kernels (parallel/ep.py::route_forward): [pre-MoE norm + router + dispatch] -> grouped
             # gate/up -> grouped down (+ return) -> [combine + next layer's input norm]; the shared experts fork onto the side
@@ -383,17 +369,14 @@ class DeepseekV2Stage(StageModel):
             def shared_branch(normed):
                 if "s_gate" not in w:
                     return h, None
-                if self.overlap_shared_experts and hasattr(O, "run_aside"):
+                if hasattr(O, "run_aside"):
                     hs = torch.empty_like(h)
                     return hs, O.run_aside(lambda: O.linear(O.gated_up(normed, w["s_gate"], w["s_up"], "silu"), w["s_down"], residual=h, out=hs))
                 return O.linear(O.gated_up(normed, w["s_gate"], w["s_up"], "silu"), w["s_down"], residual=h), None
 
             nxt = self.layer_weights.get(i + 1)
             nn = (nxt["in_ln"], c.rms_norm_eps) if (nxt is not None and "in_ln" in nxt and self.spec.runs_attn(i + 1)) else None
-            res = ep[i].route_forward(h, w["router"], dict(top_k=c.num_experts_per_tok, method=c.topk_method, n_group=c.n_group or 1,
-                                                           topk_group=c.topk_group or 1, scaling=c.routed_scaling_factor,
-                                                           norm_topk=c.norm_topk_prob),
-                                      (w["post_ln"], c.rms_norm_eps), shared_branch, next_norm=nn)
+            res = ep.route_forward(h, w["router"], rk, (w["post_ln"], c.rms_norm_eps), shared_branch, next_norm=nn)
             if nn is not None:
                 self._prenormed = res
                 return res[0]
@@ -405,7 +388,7 @@ class DeepseekV2Stage(StageModel):
                 # shared experts: h += down(silu(gate x) * up x).  Independent of the routed path until the final combine, so the
                 # CUDA backend runs the two GEMMs on a side stream (a parallel branch of the decode graph) while the main
                 # stream does router -> permutation / expert all-to-all -> expert GEMMs; the combine joins them.
-                if self.overlap_shared_experts and hasattr(O, "run_aside") and self.backend_name == "b200":
+                if hasattr(O, "run_aside") and self.backend_name == "b200":
                     hs, h_in = torch.empty_like(h), h   # result buffer allocated before the fork
                     join = O.run_aside(lambda: O.linear(O.gated_up(normed, w["s_gate"], w["s_up"], "silu"), w["s_down"],
                                                         residual=h_in, out=hs))
@@ -413,21 +396,11 @@ class DeepseekV2Stage(StageModel):
                 else:
                     h = O.linear(O.gated_up(normed, w["s_gate"], w["s_up"], "silu"), w["s_down"], residual=h)
             extra = dict(extra=w["n_fused_shared"]) if "n_fused_shared" in w else {}
-            ep = getattr(self, "ep_layers", None)
-            if hasattr(O, "moe_block") and join is None and not (ep is not None and i in ep):
-                # CUDA backend, whole bank local: router + experts as one op (scatter path for decode batches, ops/b200.py)
-                return O.moe_block(normed, w["router"], dict(top_k=c.num_experts_per_tok, method=c.topk_method, n_group=c.n_group or 1,
-                                                             topk_group=c.topk_group or 1, scaling=c.routed_scaling_factor,
-                                                             norm_topk=c.norm_topk_prob),
-                                   w["e_gate"], w["e_up"], w["e_down"], "silu", residual=h, **extra, **self._final_kwargs(i, T, "mlp"))
-            idx, wts = O.moe_route(normed, w["router"], c.num_experts_per_tok, c.topk_method,
-                                   c.n_group or 1, c.topk_group or 1, c.routed_scaling_factor,
-                                   c.norm_topk_prob, **extra)
-            ep = getattr(self, "ep_layers", None)
-            if ep is not None and i in ep:
+            idx, wts = O.moe_route(normed, w["router"], **rk, **extra)
+            if ep is not None:
                 # expert-parallel mode (parallel/ep.py): routed experts are sharded over the ranks of the NVSwitch
                 # domain, tokens travel through the fused dispatch / return kernels
-                return ep[i].forward(normed, idx, wts, residual=h, join=join)
+                return ep.forward(normed, idx, wts, residual=h, join=join)
             kw = dict(join=join) if join is not None else {}
             return O.moe_experts(normed, idx, wts, w["e_gate"], w["e_up"], w["e_down"], "silu", residual=h,
                                  **kw, **self._final_kwargs(i, T, "mlp"))

@@ -231,47 +231,6 @@ def run_aside(fn) -> _Join:
     return _Join(done)
 
 
-_aside_last = {}
-
-
-def prefetch_aside(tensors, nbytes_each: int):
-    """Start pulling the first ``nbytes_each`` bytes of every tensor into L2 on the side stream (forked from the current stream at
-    this point, NOT joined here: nothing depends on a prefetch — :func:`join_aside` ties the side stream back once per forward so
-    a graph capture ends with all its branches joined).  The main stream's kernel chain keeps its programmatic (PDL) edges."""
-    cur = torch.cuda.current_stream()
-    dev = cur.device.index
-    side = _side_streams.get(dev)
-    if side is None:
-        side = _side_streams[dev] = torch.cuda.Stream(device=cur.device)
-    fork = torch.cuda.Event()
-    fork.record(cur)
-    side.wait_event(fork)
-    with torch.cuda.stream(side):
-        for t in tensors:
-            C().l2_prefetch(t, 0, min(int(nbytes_each), t.numel() * t.element_size()) // 16 * 16)
-        done = torch.cuda.Event()
-        done.record(side)
-    _aside_last[dev] = done
-
-
-def join_aside():
-    """Join the side stream's outstanding prefetches into the current stream (end of a forward pass)."""
-    cur = torch.cuda.current_stream()
-    ev = _aside_last.pop(cur.device.index, None)
-    if ev is not None:
-        cur.wait_event(ev)
-        C().pdl_skip_next()
-
-
-def l2_prefetch_bytes() -> int:
-    """Bytes of the next MoE block's gate / up banks (each) to prefetch into L2 during a decode layer's attention chain
-    (``MLXB200_L2_PREFETCH_MB``, total across both banks; 0 = off)."""
-    try:
-        return int(float(os.environ.get("MLXB200_L2_PREFETCH_MB", "0")) * (1 << 20)) // 2
-    except ValueError:
-        return 0
-
-
 def moe_experts(x, idx, w, Wg: LinearWeight, Wu: LinearWeight, Wd: LinearWeight, act: str = "silu",
                 extra: Optional[torch.Tensor] = None, residual: Optional[torch.Tensor] = None,
                 out: Optional[torch.Tensor] = None, signal: Optional[Tuple[int, int]] = None, join: Optional[_Join] = None):
@@ -369,15 +328,12 @@ def moe_block(x, gate_w, route_kw: dict, Wg: LinearWeight, Wu: LinearWeight, Wd:
     T = x.shape[0]
     fp8 = fp8_experts_enabled(Wg) and x.shape[1] % 128 == 0
     quant = (Wg.is_quantized or Wu.is_quantized or Wd.is_quantized) and not fp8
-    if quant or T > SCATTER_MAX_TOKENS or os.environ.get("MLXB200_MOE_SCATTER", "1") == "0":
+    if quant or T > SCATTER_MAX_TOKENS:
         if pre_norm is not None:
             x = rmsnorm(x, pre_norm[0], pre_norm[1])
         idx, wts = moe_route(x, gate_w, extra=extra, **route_kw)
         res = moe_experts(x, idx, wts, Wg, Wu, Wd, act, residual=residual, out=out, signal=signal)
         return res if next_norm is None else (res, rmsnorm(res, next_norm[0], next_norm[1]))
-    fuse_norms = os.environ.get("MLXB200_FUSE_NORMS", "1") != "0"
-    if pre_norm is not None and not fuse_norms:
-        x, pre_norm = rmsnorm(x, pre_norm[0], pre_norm[1]), None
     if fp8:
         (gq, gs), (uq, us), (dq, ds) = _fp8pack(Wg), _fp8pack(Wu), _fp8pack(Wd)
         E, H = gq.shape[0], x.shape[1]
@@ -411,7 +367,7 @@ def moe_block(x, gate_w, route_kw: dict, Wg: LinearWeight, Wu: LinearWeight, Wd:
         h = c.grouped_linear(xs, wg, wu, counts, stride, ACT_IDS[act], False, None, None, None, T * k, stride)
         y = c.grouped_linear(h, wd, None, counts, stride, 0, True, None, None, None, T * k, stride)
     flag, val = signal if signal is not None else (0, 0)
-    if next_norm is not None and signal is None and fuse_norms and H <= 8192:
+    if next_norm is not None and signal is None and H <= 8192:
         normed = torch.empty(T, H, dtype=torch.bfloat16, device=x.device)
         res = c.moe_combine(y, pair_row, wts, residual, out, int(k), 0, 0, counts, _bf16(next_norm[0]), float(next_norm[1]), normed)
         return res, normed

@@ -73,10 +73,8 @@ int sm_count() {
 }
 
 // Token tile of the grouped (MoE) GEMMs: ~2x the average rows per expert but never below 64, so an expert's rows rarely need a
-// second tile; gemm_clamp_bn caps it at what the register accumulators allow.  MLXB200_GROUPED_BN=<n> overrides (tuning).
+// second tile; gemm_clamp_bn caps it at what the register accumulators allow.
 int grouped_bn(int64_t max_rows, int64_t R, int64_t E) {
-  static const int forced = [] { const char* e = std::getenv("MLXB200_GROUPED_BN"); return e ? std::atoi(e) : 0; }();
-  if (forced > 0) return b200::gemm_pick_bn((int)std::min<int64_t>(max_rows, forced));
   return b200::gemm_pick_bn((int)std::min<int64_t>(max_rows, std::max<int64_t>(64, 2 * ((R + E - 1) / E))));
 }
 
@@ -85,12 +83,8 @@ int auto_splits(int rows, int n, int k, bool grouped) {
   const int tiles = (n + 127) / 128;
   const int kb = (k + 63) / 64;
   int s = 1;
-  // fill ~one wave of SMs while keeping >= 8 k-blocks per split ...
+  // fill ~one wave of SMs while keeping >= 8 k-blocks per split
   while (tiles * (s * 2) <= sm_count() && kb / (s * 2) >= 8 && s < 4) s *= 2;
-  // ... and for long reductions over few feature tiles (the folded MLA output projection: 16 tiles x 128 k-blocks) go to the
-  // full portable cluster of 8 splits: 64 CTAs stream at ~100 GB/s each, so the kernel is per-SM-bandwidth bound below that
-  static const bool split8 = [] { const char* e = std::getenv("MLXB200_SPLIT8"); return e != nullptr && e[0] == '1'; }();  // measured slower (0.12 ms / step): opt-in
-  if (split8 && s == 4 && tiles * 8 <= sm_count() && kb / 8 >= 16) s = 8;
   return s;
 }
 
@@ -214,9 +208,8 @@ Tensor linear_q(const Tensor& x, const Tensor& wq, const Tensor& scales_t, const
   if (bias.has_value()) { check_bf16(*bias, "bias"); a.bias = bias->data_ptr(); }
   a.act = (int)act; a.softcap = (float)softcap;
   // quantised weights: 3.5x fewer bytes per tile, so batches of >= 64 tokens use the persistent kernel un-split; tiny decode
-  // batches are latency-bound per tile like the bf16 path and take the same split-K heuristic (MLXB200_Q_SPLITK=0 disables)
-  static const bool q_splitk = [] { const char* e = std::getenv("MLXB200_Q_SPLITK"); return !(e && e[0] == '0'); }();
-  int sp = splits > 0 ? (int)splits : ((q_splitk && T <= 32) ? auto_splits((int)T, (int)N, (int)K, false) : 1);
+  // batches are latency-bound per tile like the bf16 path and take the same split-K heuristic
+  int sp = splits > 0 ? (int)splits : (T <= 32 ? auto_splits((int)T, (int)N, (int)K, false) : 1);
   a.splits = sp;
   auto& sc = scratch();
   Tensor ctr = sc.get_counters(x.device());
@@ -288,12 +281,6 @@ void rope_(Tensor x, const Tensor& positions, const Tensor& inv_freq, int64_t ro
   const c10::cuda::CUDAGuard guard(x.device());
   LAUNCH_OK(b200::rope_launch(x.data_ptr(), x.stride(0), x.stride(1), (int)x.size(1), positions.data_ptr<int>(), inv_freq.data_ptr<float>(),
                             (int)rot_off, (int)rot_dim, interleaved, (float)mscale, (int)x.size(0), cur_stream()));
-}
-
-void l2_prefetch(const Tensor& t, int64_t offset_bytes, int64_t nbytes) {
-  TORCH_CHECK(t.is_cuda() && t.is_contiguous() && offset_bytes >= 0 && nbytes >= 0 && offset_bytes + nbytes <= (int64_t)t.nbytes(), "bad prefetch range");
-  const c10::cuda::CUDAGuard guard(t.device());
-  LAUNCH_OK(b200::l2_prefetch_launch(static_cast<const char*>(t.data_ptr()) + offset_bytes, (unsigned long long)nbytes, cur_stream()));
 }
 
 Tensor embed(const Tensor& ids, const Tensor& table, const c10::optional<Tensor>& scales, const c10::optional<Tensor>& biases,
@@ -811,7 +798,6 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("rmsnorm", &rmsnorm, py::arg("x"), py::arg("w"), py::arg("eps"), py::arg("gemma") = false, py::arg("residual") = py::none(),
         py::arg("out") = py::none(), py::arg("signal_flag_ptr") = 0, py::arg("signal_value") = 0);
   m.def("rope_", &rope_);
-  m.def("l2_prefetch", &l2_prefetch, py::arg("t"), py::arg("offset_bytes"), py::arg("nbytes"));
   m.def("embed", &embed, py::arg("ids"), py::arg("table"), py::arg("scales") = py::none(), py::arg("biases") = py::none(),
         py::arg("bits") = 0, py::arg("group") = 64, py::arg("scale") = 1.0);
   m.def("kv_write", &kv_write);

@@ -12,8 +12,6 @@ cudaError_t rmsnorm_launch(const void* x, long long ld_x, const void* w, const v
                            uint32_t signal_value = 0, unsigned int* done_counter = nullptr);
 cudaError_t rope_launch(void* x, long long ld_t, long long ld_h, int heads, const int* positions, const float* inv_freq,
                         int rot_off, int rot_dim, bool interleaved, float mscale, int T, cudaStream_t s);
-// bulk L2 prefetch of [p, p + bytes) (16 B aligned), a few threads, no PDL: meant for a side stream
-cudaError_t l2_prefetch_launch(const void* p, unsigned long long bytes, cudaStream_t s);
 cudaError_t embed_launch(const long long* ids, const void* table, const void* scales, const void* biases, int bits, int group,
                          void* out, int H, float scale, int T, cudaStream_t s);
 cudaError_t kv_write_launch(const void* k, long long k_ld_t, long long k_ld_h, const void* v, long long v_ld_t,

@@ -11,21 +11,11 @@
 // produced by a predecessor), so the HBM latency of a small GEMM hides behind the kernel in front of it.
 // (launch_dependents only takes effect once *every* block of N has issued it, i.e. once all of N's blocks are
 // resident, so the waiting blocks of N+1 can never starve N; completion of N+1 implies completion of N, so N+2's
-// wait on N+1 transitively orders it after N.)  Set MLXB200_PDL=0 to fall back to plain stream-ordered launches.
+// wait on N+1 transitively orders it after N.)
 #pragma once
 #include <cuda_runtime.h>
-#include <cstdlib>
 
 namespace b200 {
-
-inline bool pdl_enabled() {
-  static int v = -1;
-  if (v < 0) {
-    const char* e = std::getenv("MLXB200_PDL");
-    v = (e != nullptr && e[0] == '0') ? 0 : 1;
-  }
-  return v != 0;
-}
 
 // One-shot opt-out for the next launch of this host thread: the first kernel after a cross-stream fork / join has a
 // dependency that is not its same-stream predecessor, so it is launched with plain (full) dependencies.
@@ -35,7 +25,7 @@ inline bool& pdl_skip_next_flag() {
 }
 inline bool pdl_use_now() {
   bool& skip = pdl_skip_next_flag();
-  const bool use = pdl_enabled() && !skip;
+  const bool use = !skip;
   skip = false;
   return use;
 }
