@@ -4,6 +4,11 @@
 //
 // Roles (160 threads): warps 0..3 = MMA warpgroup + epilogue, warp 4 = TMA producer.
 // Barriers: full/empty per ring stage.
+//
+// Shared memory is the TMA ring plus one output staging tile; the epilogue works on the wgmma fragments in registers, so no fp32
+// accumulator tile competes with the ring (5 stages for the gate/up pair at BN = 64, 8 for a single matrix).  Token tiles are
+// loaded in 16-row boxes, only as many as the tile has valid rows: a routed expert of a decode step holds a handful of rows of its
+// 64-row segment.
 #include <algorithm>
 
 #include "gemm_common.cuh"
@@ -16,10 +21,17 @@ using namespace gemm;
 
 namespace {
 
+constexpr int kXBoxRows = 16;                             // token rows per TMA box
+constexpr int kXBoxBytes = kXBoxRows * kBlockK * 2;       // 2 KB
+
 __host__ __device__ constexpr int p_stg_rows(int BN) { return BN < 64 ? BN : 64; }
-__host__ __device__ constexpr int p_staging_bytes(int BN, int out_bytes) { return p_stg_rows(BN) * kTileM * out_bytes; }
+// Staging row pitch in elements: 16 B of padding per token row.  A fragment store writes 8 consecutive features of 4 token columns
+// (2 apart); unpadded, those columns are a multiple of 512 B apart and hit the same banks (4-way conflict), padded they are 32 B apart.
+__host__ __device__ constexpr int p_stg_ld(int out_bytes) { return kTileM + 16 / out_bytes; }
+__host__ __device__ constexpr int p_staging_bytes(int BN, int out_bytes) { return p_stg_rows(BN) * p_stg_ld(out_bytes) * out_bytes; }
 __host__ __device__ constexpr int p_num_stages(int BN, bool dual, int out_bytes) {
-  int s = (225 * 1024 - acc_bytes(BN, dual) - p_staging_bytes(BN, out_bytes) - 512) / stage_bytes(BN, dual);
+  // 227 KB opt-in shared memory less the 1 KB alignment slack, the staging tile and the barriers (at most 8 stages x 2 x 8 B)
+  int s = (227 * 1024 - 1024 - p_staging_bytes(BN, out_bytes) - 2 * 8 * 8) / stage_bytes(BN, dual);
   return s > 8 ? 8 : s;
 }
 
@@ -81,21 +93,37 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_
   constexpr int STAGES = p_num_stages(BN, DUAL, sizeof(OutT));
   constexpr int STAGE_BYTES = stage_bytes(BN, DUAL);
   constexpr int STG_ROWS = p_stg_rows(BN);
+  constexpr int STG_LD = p_stg_ld(sizeof(OutT));
+  constexpr int OFF_X = kATileBytes * (DUAL ? 2 : 1);   // token tile within a stage
   static_assert(STAGES >= 2, "ring too small");
+  static_assert(BN % kXBoxRows == 0, "token tile must be whole boxes");
 
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   // 1024 B alignment by *pointer arithmetic* on the __shared__ array: an integer round-trip loses the address space and
   // turns every LDS/STS below into a generic LD.E/ST.E (checked with cuobjdump -sass)
   uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-  float* acc_smem = reinterpret_cast<float*>(smem + STAGES * STAGE_BYTES);   // [BN * (1 + DUAL)][128] fp32
-  OutT* stg = reinterpret_cast<OutT*>(smem + STAGES * STAGE_BYTES + acc_bytes(BN, DUAL));
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES + acc_bytes(BN, DUAL) + p_staging_bytes(BN, sizeof(OutT)));
+  OutT* stg = reinterpret_cast<OutT*>(smem + STAGES * STAGE_BYTES);   // [STG_ROWS][STG_LD]
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + STAGES * STAGE_BYTES + p_staging_bytes(BN, sizeof(OutT)));
   uint64_t* empty_bar = full_bar + STAGES;
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
+  const int kb_total = (p.k + kBlockK - 1) / kBlockK;
   const bool pdl_early = p.expert_offsets != nullptr;
-  if (pdl_early) pdl_wait();
+  if (pdl_early) {
+    // Grouped launches read the router's counts, so they wait for the predecessor before anything else.  The weights do not depend
+    // on it: the producer first prefetches the first ring-full of k-blocks of this CTA's first tile into L2, so HBM streams through
+    // the router (or the gate/up -> down boundary) instead of idling.  No ring bookkeeping: the loads after the wait hit L2.
+    if (warp == kProducerWarp && elect_one()) {
+      const int w_row = (blockIdx.x / (tiles_n * tiles_m)) * p.n + (blockIdx.x % tiles_n) * kTileM;
+      const int kb_pre = kb_total < STAGES ? kb_total : STAGES;
+      for (int kb = 0; kb < kb_pre; ++kb) {
+        tma_prefetch_l2_2d(&tmap_w, kb * kBlockK, w_row);
+        if (DUAL) tma_prefetch_l2_2d(&tmap_w2, kb * kBlockK, w_row);
+      }
+    }
+    pdl_wait();
+  }
   if (p.ep_arrive != nullptr) {
     // Expert-parallel receive side: the token rows, their return addresses and the per-expert row counts of this step are written
     // into this rank's buffers by the *other ranks'* dispatch kernels.  Each source publishes the step's sequence number with
@@ -138,11 +166,17 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_
   // PDL: let the successor's CTAs become resident now (their pre-wait prologue / weight prefetch overlaps this kernel)
   pdl_launch_dependents();
 
-  const int kb_total = (p.k + kBlockK - 1) / kBlockK;
-
   if (warp == kProducerWarp) {
     // ============================================================== TMA producer
     if (elect_one()) {  // one elected lane: uniform-datapath issue, no per-instruction ELECT loop (ptx.cuh)
+      // Only the 16-row boxes that hold valid rows are loaded; the token rows of the stage beyond them keep stale data, which only
+      // feeds accumulator columns the epilogue never stores.
+      auto x_boxes = [](const TileInfo& ti) { return (ti.rows_valid + kXBoxRows - 1) / kXBoxRows; };
+      auto stage_tx = [&](const TileInfo& ti) { return (uint32_t)(OFF_X + x_boxes(ti) * kXBoxBytes); };
+      auto load_x = [&](uint8_t* st, uint64_t* bar, int kc, const TileInfo& ti) {
+        const int nb = x_boxes(ti);
+        for (int b = 0; b < nb; ++b) tma_load_2d(st + OFF_X + b * kXBoxBytes, &tmap_x, bar, kc, ti.row_base + b * kXBoxRows, kEvictLast);
+      };
       // Weights never depend on a predecessor kernel: the first ring-full of weight tiles is requested *before*
       // griddepcontrol.wait (HBM latency overlaps the predecessor's tail); the activation tiles follow after it.
       // (un-grouped launches only: iteration i <-> tile blockIdx.x + (i / kb_total) * gridDim.x, k-block i % kb_total)
@@ -154,7 +188,7 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_
           const TileInfo ti = decode_tile(p, t, tiles_n, tiles_m, BN);
           uint8_t* st = smem + pre * STAGE_BYTES;
           const int kc = (int)(pre % kb_total) * kBlockK;
-          mbar_arrive_expect_tx(&full_bar[pre], STAGE_BYTES);
+          mbar_arrive_expect_tx(&full_bar[pre], stage_tx(ti));
           tma_load_2d(st, &tmap_w, &full_bar[pre], kc, ti.w_row, kEvictFirst);
           if (DUAL) tma_load_2d(st + kATileBytes, &tmap_w2, &full_bar[pre], kc, ti.w_row, kEvictFirst);
         }
@@ -162,8 +196,7 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_
         for (uint32_t i = 0; i < pre; ++i) {
           const int t = blockIdx.x + (int)(i / kb_total) * gridDim.x;
           const TileInfo ti = decode_tile(p, t, tiles_n, tiles_m, BN);
-          tma_load_2d(smem + i * STAGE_BYTES + kATileBytes * (DUAL ? 2 : 1), &tmap_x, &full_bar[i], (int)(i % kb_total) * kBlockK,
-                      ti.row_base, kEvictLast);
+          load_x(smem + i * STAGE_BYTES, &full_bar[i], (int)(i % kb_total) * kBlockK, ti);
         }
       }
       uint32_t it = 0;
@@ -176,16 +209,15 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_
           mbar_wait(&empty_bar[s], ph ^ 1);
           uint8_t* st = smem + s * STAGE_BYTES;
           const int kc = kb * kBlockK;
-          mbar_arrive_expect_tx(&full_bar[s], STAGE_BYTES);
+          mbar_arrive_expect_tx(&full_bar[s], stage_tx(ti));
           tma_load_2d(st, &tmap_w, &full_bar[s], kc, ti.w_row, kEvictFirst);
           if (DUAL) tma_load_2d(st + kATileBytes, &tmap_w2, &full_bar[s], kc, ti.w_row, kEvictFirst);
-          tma_load_2d(st + kATileBytes * (DUAL ? 2 : 1), &tmap_x, &full_bar[s], kc, ti.row_base, kEvictLast);
+          load_x(st, &full_bar[s], kc, ti);
         }
       }
     }
   } else {
     // ============================================================== MMA warpgroup, then epilogue (128 threads)
-    const int f_local = threadIdx.x;
     const int et = threadIdx.x;
     constexpr int kVec = 8, kChunks = kTileM / kVec, kRowsPerIter = kEpiThreads / kChunks;
     uint32_t it = 0, tc = 0, my_tiles = 0;
@@ -199,36 +231,37 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_
       float acc[2][BN / 2], acc2[2][BN / 2];
       acc_zero<BN>(acc);
       if (DUAL) acc_zero<BN>(acc2);
-      mma_mainloop<BN, DUAL, STAGES, STAGE_BYTES, kATileBytes * (DUAL ? 2 : 1)>(
+      mma_mainloop<BN, DUAL, STAGES, STAGE_BYTES, OFF_X>(
           acc, acc2, smem, empty_bar, it, kb_total, [&](uint32_t s, uint32_t ph) { mbar_wait(&full_bar[s], ph); });
       it += kb_total;
-      acc_store_smem<BN>(acc, acc_smem, 0);
-      if (DUAL) acc_store_smem<BN>(acc2, acc_smem, BN);
       if (!waited) {  // residual / out are ordered after the predecessor
         pdl_wait();
         waited = true;
       }
-      named_bar_sync(1, kEpiThreads);
-      const int f_glob = ti.n0 + f_local;
-      const float bias = (p.bias != nullptr && f_glob < p.n) ? __bfloat162float(p.bias[f_glob]) : 0.0f;
-#pragma unroll 1
+      // this thread's fragment rows (features) are h * 64 + wg_row(j), and wg_row(j) only depends on bit 1 of j
+      float bias[2][2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int r = 0; r < 2; ++r) {
+          const int f_glob = ti.n0 + h * 64 + wg_row(2 * r);
+          bias[h][r] = (p.bias != nullptr && f_glob < p.n) ? __bfloat162float(p.bias[f_glob]) : 0.0f;
+        }
+      // Epilogue on the fragments: acc[h][j] and acc2[h][j] are the same (feature, token).  The chunk loop is unrolled so that the
+      // fragment index stays a compile-time constant (the accumulators never leave registers); only valid token columns are stored.
+#pragma unroll
       for (int c0 = 0; c0 < BN; c0 += STG_ROWS) {
         if (c0 >= ti.rows_valid) break;
-#pragma unroll 1
-        for (int c = c0; c < c0 + STG_ROWS; c += 16) {
-          if (c >= ti.rows_valid) break;
-          float g[16], u[16];
 #pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            g[j] = acc_smem[(c + j) * kTileM + f_local];
-            if (DUAL) u[j] = acc_smem[(BN + c + j) * kTileM + f_local];
-          }
+        for (int j = c0 / 2; j < (c0 + STG_ROWS) / 2; ++j) {
+          const int c = wg_col(j);
+          if (c >= ti.rows_valid) continue;
 #pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            float y = g[j] + bias;
-            if (DUAL) y = apply_act(p.act, y) * u[j];
+          for (int h = 0; h < 2; ++h) {
+            float y = acc[h][j] + bias[h][(j >> 1) & 1];
+            if (DUAL) y = apply_act(p.act, y) * acc2[h][j];
             if (p.softcap > 0.f) y = p.softcap * tanhf(y / p.softcap);
-            stage_store<OutT>(&stg[(c - c0 + j) * kTileM + f_local], y);
+            stage_store<OutT>(&stg[(c - c0) * STG_LD + h * 64 + wg_row(j)], y);
           }
         }
         named_bar_sync(1, kEpiThreads);
@@ -240,13 +273,13 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_
             const size_t row = static_cast<size_t>(ti.row_base + c0 + r);
             float vals[kVec];
             if (sizeof(OutT) == 2) {
-              const uint4 raw = *reinterpret_cast<const uint4*>(reinterpret_cast<const __nv_bfloat16*>(stg) + r * kTileM + ch * kVec);
+              const uint4 raw = *reinterpret_cast<const uint4*>(reinterpret_cast<const __nv_bfloat16*>(stg) + r * STG_LD + ch * kVec);
               const uint32_t w4[4] = {raw.x, raw.y, raw.z, raw.w};
 #pragma unroll
               for (int j = 0; j < 4; ++j) { vals[2 * j] = bf16_lo(w4[j]); vals[2 * j + 1] = bf16_hi(w4[j]); }
             } else {
-              const float4 a = *reinterpret_cast<const float4*>(reinterpret_cast<const float*>(stg) + r * kTileM + ch * kVec);
-              const float4 b = *reinterpret_cast<const float4*>(reinterpret_cast<const float*>(stg) + r * kTileM + ch * kVec + 4);
+              const float4 a = *reinterpret_cast<const float4*>(reinterpret_cast<const float*>(stg) + r * STG_LD + ch * kVec);
+              const float4 b = *reinterpret_cast<const float4*>(reinterpret_cast<const float*>(stg) + r * STG_LD + ch * kVec + 4);
               vals[0] = a.x; vals[1] = a.y; vals[2] = a.z; vals[3] = a.w;
               vals[4] = b.x; vals[5] = b.y; vals[6] = b.z; vals[7] = b.w;
             }
@@ -271,7 +304,7 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_
             }
           }
         }
-        named_bar_sync(1, kEpiThreads);  // staging buffer (and, after the last chunk, the accumulator) free again
+        named_bar_sync(1, kEpiThreads);  // staging buffer free again
       }
       ++my_tiles;
       ++tc;
@@ -304,7 +337,7 @@ template <int BN, bool DUAL, typename OutT>
 cudaError_t p_launch_one(const CUtensorMap& tw, const CUtensorMap& tw2, const CUtensorMap& tx, const GemmParams& p, int tiles_n,
                          int tiles_m, int num_tiles, cudaStream_t stream) {
   constexpr int STAGES = p_num_stages(BN, DUAL, sizeof(OutT));
-  constexpr int smem = STAGES * stage_bytes(BN, DUAL) + acc_bytes(BN, DUAL) + p_staging_bytes(BN, sizeof(OutT)) + 2 * STAGES * 8 + 1024;
+  constexpr int smem = STAGES * stage_bytes(BN, DUAL) + p_staging_bytes(BN, sizeof(OutT)) + 2 * STAGES * 8 + 1024;
   static_assert(smem <= 227 * 1024, "shared memory budget exceeded");
   auto kern = gemm_persistent_kernel<BN, DUAL, OutT>;
   static bool configured = false;
@@ -350,7 +383,7 @@ cudaError_t gemm_persistent_launch(const GemmArgs& a, cudaStream_t stream) {
   } else {
     tw2 = tw;
   }
-  if (!gemm_make_tmap(&tx, a.x, a.x_rows, a.k, a.ld_x, bn)) return cudaErrorUnknown;
+  if (!gemm_make_tmap(&tx, a.x, a.x_rows, a.k, a.ld_x, kXBoxRows)) return cudaErrorUnknown;
 
   GemmParams p;
   p.row_dst = nullptr; p.signal_peers = nullptr; p.num_signal_peers = 0; p.w_sf = p.w2_sf = p.x_sf = nullptr; p.sf_ld_w = p.sf_ld_x = 0;

@@ -72,6 +72,11 @@ B200_DEVICE void tma_load_2d(void* smem_dst, const CUtensorMap* m, uint64_t* bar
       ::"r"(smem_u32(smem_dst)), "l"(reinterpret_cast<uint64_t>(m)), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "l"(hint)
       : "memory");
 }
+// 2-D tile prefetch global -> L2 only: no shared-memory destination and no mbarrier, so nothing waits on it
+B200_DEVICE void tma_prefetch_l2_2d(const CUtensorMap* m, int c0, int c1) {
+  asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global.tile [%0, {%1, %2}];" ::"l"(reinterpret_cast<uint64_t>(m)), "r"(c0), "r"(c1)
+               : "memory");
+}
 B200_DEVICE void fence_proxy_async_smem() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 // ---------------------------------------------------------------------------------------------- wgmma
