@@ -23,7 +23,7 @@ import torch
 
 from ..ops.meta import BatchMeta
 from .kv_cache import PageAllocator, PrefixCache, SequenceTable
-from .sampler import SamplingParams
+from .sampler import OutputCounts, SamplingParams, check_penalty_table
 
 
 # ---------------------------------------------------------------------------------------------
@@ -40,6 +40,9 @@ class StepInput:
     sample_mask: List[bool]         # False for non-final prefill chunks
     is_prefill: bool
     rng: Optional[List[tuple]] = None   # per sequence: (seed, tokens sampled so far) — the sampler's random stream of that request
+    # per sequence: output token counts of requests with a presence / frequency penalty (else None); None when no
+    # request of the engine uses one
+    counts: Optional[List[Optional[OutputCounts]]] = None
 
 
 @dataclass
@@ -71,6 +74,8 @@ class Request:
         self.eos_token_id = eos_token_id
         self.stop_id_sequences = stop_id_sequences or []
         self.output: List[int] = []
+        # times each token id occurs in ``output``: kept only for the presence / frequency penalties
+        self.counts: Optional[OutputCounts] = OutputCounts() if params.uses_output_penalty else None
         self.events: "queue.SimpleQueue[TokenEvent]" = queue.SimpleQueue()   # C implementation: one put per generated token
         self.finished = False
         self.finish_reason: Optional[str] = None
@@ -141,6 +146,7 @@ class LLMEngine:
         self._wake = threading.Event()
         self.stats = dict(steps=0, prefill_tokens=0, decode_tokens=0, finished=0, prefix_cached_tokens=0)
         self.sinks: list = []      # event sinks of the API worker processes (server/frontend.py): flushed once per scheduler iteration
+        self._penalised = 0        # running requests with a presence / frequency penalty (their steps carry output counts)
 
     # -------------------------------------------------------------------------- public API
     def submit(self, prompt: Sequence[int], params: Optional[SamplingParams] = None, max_tokens: int = 100,
@@ -149,6 +155,7 @@ class LLMEngine:
         (server/frontend.py) passes a per-worker sink so a step's tokens leave the engine process as one message."""
         params = params or SamplingParams()
         params.validate()
+        check_penalty_table(params, max_tokens)
         if len(prompt) == 0:
             raise ValueError("empty prompt")
         if len(prompt) + max_tokens > self.max_model_len:
@@ -242,6 +249,7 @@ class LLMEngine:
                 self.table.release(r.id)
                 r.events.put(None)
             self.groups[g] = []
+        self._penalised = 0
         for s in self.sinks:
             s.flush()
 
@@ -279,6 +287,8 @@ class LLMEngine:
                 self.stats["prefix_cached_tokens"] += n
             self.table.reserve(r.id, len(r.prompt) - r.prefilled + r.max_tokens)
             self.groups[g].append(r)
+            if r.counts is not None:
+                self._penalised += 1
 
     def _build_step(self, g: int) -> Optional[StepInput]:
         reqs = [r for r in self.groups[g] if not r.finished]
@@ -322,14 +332,18 @@ class LLMEngine:
         meta = BatchMeta.build(q_lens, ctx0, bts, self.page_size, pad_blocks_to=width)
         ctxs = [(r.prompt + r.output)[-max(1, r.params.repetition_context_size):]
                 if r.params.repetition_penalty not in (0, 1.0) else [] for r in seqs]
+        counts = [r.counts for r in seqs] if self._penalised else None
         return StepInput(g, [r.id for r in seqs], torch.tensor(toks, dtype=torch.int64), meta,
-                         [r.params for r in seqs], ctxs, mask, is_prefill, [(r.seed, len(r.output)) for r in seqs]), seqs, q_lens
+                         [r.params for r in seqs], ctxs, mask, is_prefill, [(r.seed, len(r.output)) for r in seqs],
+                         counts), seqs, q_lens
 
     def _finish(self, r: Request, reason: str):
         r.finished, r.finish_reason = True, reason
         r.t_done = time.perf_counter()
         self.table.release(r.id)
         self.stats["finished"] += 1
+        if r.counts is not None:
+            self._penalised -= 1
 
     def _process(self, g: int, seqs: List[Request], q_lens: List[int], inp: StepInput, out: StepOutput):
         length, n_decode = self.table.length, 0
@@ -352,6 +366,8 @@ class LLMEngine:
             if r.t_first is None:
                 r.t_first = time.perf_counter()
             r.output.append(tok)
+            if r.counts is not None:
+                r.counts.add(tok)
             top = None
             if r.params.logprobs > 0 and out.top_ids is not None:
                 k = r.params.logprobs

@@ -111,10 +111,12 @@ cudaError_t apply_penalties_launch(float* logits, int B, int V, const int* rep_c
 // tokens/logprob per row; temperature==0 -> argmax, top_p in (0,1) -> nucleus; Philox-style counter RNG
 // row_rng (optional, device): per-row [seed, step] pairs that override the scalars (graph-replay safe);
 // tag_src/tag_dst (optional): 16 bytes copied verbatim next to the results (scheduler step id)
-cudaError_t sample_launch(const float* logits, int B, int V, const float* temperature, const float* top_p,
-                          unsigned long long seed, unsigned long long step, const unsigned long long* row_rng, long long* tokens,
-                          float* logprobs, int top_k, long long* top_ids, float* top_lp, const void* tag_src, void* tag_dst,
-                          cudaStream_t s);
+// keep_k / min_p (optional, device, [B]): per-row top-k (0 or >= V = off) and min-p (0 = off) filters of the temperature draw;
+// a null pointer or an off value leaves the row on the plain top-p / categorical path
+cudaError_t sample_launch(const float* logits, int B, int V, const float* temperature, const float* top_p, const int* keep_k,
+                          const float* min_p, unsigned long long seed, unsigned long long step, const unsigned long long* row_rng,
+                          long long* tokens, float* logprobs, int top_k, long long* top_ids, float* top_lp, const void* tag_src,
+                          void* tag_dst, cudaStream_t s);
 
 // ---- p2p.cu
 cudaError_t wait_flag_launch(const uint32_t* flag, uint32_t expected, uint32_t* error_flag, cudaStream_t s);

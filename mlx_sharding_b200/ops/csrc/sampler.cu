@@ -5,6 +5,9 @@
 // keep tokens whose cumulative mass exceeds 1 - top_p); here the nucleus is found without a sort by
 // bisection on the logit threshold, and sampling inside it uses the Gumbel-max trick with a
 // counter-based RNG (stateless: seed, step, row, token id).
+// Optional per-row filters, in the order top-k -> top-p -> min-p: top-k keeps the logits >= the exact k-th largest (radix select,
+// ties kept) and restricts the nucleus to that set; min-p is one logit threshold.  Presence / frequency penalties arrive folded
+// into the additive bias table of apply_penalties_kernel.
 #include "kernels.h"
 #include "launch.h"
 #include "ptx.cuh"
@@ -56,8 +59,110 @@ __device__ float block_sum(float x, float* sm) {
   return r;
 }
 
-__global__ void __launch_bounds__(kSampThreads)
+// fp32 -> uint32 key with the same order (negative values flipped, positive ones offset above them); -inf is the smallest key
+__device__ __forceinline__ uint32_t order_key(float x) {
+  const uint32_t u = __float_as_uint(x);
+  return (u & 0x80000000u) ? ~u : (u | 0x80000000u);
+}
+__device__ __forceinline__ float key_value(uint32_t k) {
+  return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
+}
+
+constexpr int kRadixBins = 2048;
+
+// Exact k-th largest logit of a row (1 <= k < V) by radix select over `order_key`: three passes of 11, 11 and 10 bits, each a
+// shared-memory histogram of the keys that match the digits chosen so far, then a suffix scan that finds the digit holding the
+// k-th key. `hist` has kRadixBins words, `sm_u` 34.
+__device__ float radix_kth_largest(const float* __restrict__ lg, int V, int k, uint32_t* hist, uint32_t* sm_u) {
+  const int t = threadIdx.x, warp = t >> 5, lane = t & 31;
+  uint32_t prefix = 0, mask = 0, rem = (uint32_t)k;  // rem: rank of the wanted key among the keys that match `prefix`
+#pragma unroll 1
+  for (int pass = 0; pass < 3; ++pass) {
+    const int shift = pass == 0 ? 21 : (pass == 1 ? 10 : 0);
+    const uint32_t dmask = pass == 2 ? 1023u : 2047u;
+    for (int i = t; i < kRadixBins; i += kSampThreads) hist[i] = 0u;
+    __syncthreads();
+    for (int i = t; i < V; i += kSampThreads) {
+      const uint32_t key = order_key(lg[i]);
+      if ((key & mask) == prefix) atomicAdd(&hist[(key >> shift) & dmask], 1u);
+    }
+    __syncthreads();
+    // thread t owns bins hi = 2047 - 2t and lo = 2046 - 2t: a scan in thread order counts keys from the top bin down
+    const uint32_t ch = hist[kRadixBins - 1 - 2 * t], cl = hist[kRadixBins - 2 - 2 * t];
+    uint32_t incl = ch + cl;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const uint32_t y = __shfl_up_sync(0xffffffffu, incl, o);
+      if (lane >= o) incl += y;
+    }
+    if (lane == 31) sm_u[warp] = incl;
+    __syncthreads();
+    uint32_t above = incl - ch - cl;  // keys in bins above `hi`
+    for (int w = 0; w < warp; ++w) above += sm_u[w];
+    if (above < rem && above + ch >= rem) {
+      sm_u[32] = kRadixBins - 1 - 2 * t;
+      sm_u[33] = rem - above;
+    } else if (above + ch < rem && above + ch + cl >= rem) {
+      sm_u[32] = kRadixBins - 2 - 2 * t;
+      sm_u[33] = rem - above - ch;
+    }
+    __syncthreads();
+    prefix |= sm_u[32] << shift;
+    mask |= dmask << shift;
+    rem = sm_u[33];
+  }
+  return key_value(prefix);
+}
+
+// Temperature draw of one row inside the kept set.  kFilt == false is the plain top-p / categorical path; kFilt == true adds the
+// top-k floor `kth` (the top-p mass sums run over x >= kth only) and keeps x >= floor = max(kth, min-p threshold) in the draw.
+template <bool kFilt>
+__device__ __forceinline__ int draw_token(const float* __restrict__ lg, int V, float amv, float temp, float tp, float kth,
+                                          float floor, unsigned long long seed, unsigned long long step, uint32_t rng_row,
+                                          ArgMax* sm_a, float* sm_f) {
+  const float inv_t = 1.0f / temp;
+  float thresh = -INFINITY;  // keep logits > thresh
+  if (tp > 0.f && tp < 1.f) {
+    // Z at temperature
+    float zs = 0.f;
+    for (int i = threadIdx.x; i < V; i += kSampThreads) {
+      const float x = lg[i];
+      if (!kFilt || x >= kth) zs += __expf((x - amv) * inv_t);
+    }
+    zs = block_sum(zs, sm_f);
+    // bisection on x in [lo, hi]: F(x) = mass{logit <= x}; find the smallest kept logit, i.e. the
+    // infimum of x with F(x) > 1 - top_p
+    float lo = amv - 80.f * temp, hi = amv;
+    const float target = (1.0f - tp) * zs;
+    for (int it = 0; it < 26; ++it) {
+      const float mid = 0.5f * (lo + hi);
+      float ms = 0.f;
+      for (int i = threadIdx.x; i < V; i += kSampThreads) {
+        const float x = lg[i];
+        if (x <= mid && (!kFilt || x >= kth)) ms += __expf((x - amv) * inv_t);
+      }
+      ms = block_sum(ms, sm_f);
+      if (ms > target) hi = mid; else lo = mid;
+    }
+    thresh = lo;  // F(lo) <= target < F(hi): everything strictly above lo is in the nucleus
+  }
+  // Gumbel-max over the kept set: argmax (logit / T + g), g = -log(-log(u))
+  ArgMax gm{-INFINITY, 0x7fffffff};
+  for (int i = threadIdx.x; i < V; i += kSampThreads) {
+    const float x = lg[i];
+    if (x > thresh && (!kFilt || x >= floor)) {
+      const float u = uniform01(seed, step, rng_row, i);
+      const float g = -__logf(-__logf(u));
+      gm = better(gm, ArgMax{(x - amv) * inv_t + g, i});
+    }
+  }
+  gm = block_argmax(gm, sm_a);
+  return gm.i;
+}
+
+__global__ void __launch_bounds__(kSampThreads, 1)
 sample_kernel(const float* __restrict__ logits, int V, const float* __restrict__ temperature, const float* __restrict__ top_p,
+              const int* __restrict__ keep_k, const float* __restrict__ min_p,
               unsigned long long seed, unsigned long long step, const unsigned long long* __restrict__ row_rng,
               long long* __restrict__ tokens, float* __restrict__ logprobs, int top_k, long long* __restrict__ top_ids,
               float* __restrict__ top_lp, const uint4* __restrict__ tag_src, uint4* __restrict__ tag_dst) {
@@ -91,41 +196,20 @@ sample_kernel(const float* __restrict__ logits, int V, const float* __restrict__
   const float tp = top_p[b];
   int token = am.i;
   if (temp > 0.f) {
-    const float inv_t = 1.0f / temp;
-    float thresh = -INFINITY;  // keep logits > thresh
-    if (tp > 0.f && tp < 1.f) {
-      // Z at temperature
-      float zs = 0.f;
-      for (int i = threadIdx.x; i < V; i += kSampThreads) zs += __expf((lg[i] - am.v) * inv_t);
-      zs = block_sum(zs, sm_f);
-      // bisection on x in [lo, hi]: F(x) = mass{logit <= x}; find the smallest kept logit, i.e. the
-      // infimum of x with F(x) > 1 - top_p
-      float lo = am.v - 80.f * temp, hi = am.v;
-      const float target = (1.0f - tp) * zs;
-      for (int it = 0; it < 26; ++it) {
-        const float mid = 0.5f * (lo + hi);
-        float ms = 0.f;
-        for (int i = threadIdx.x; i < V; i += kSampThreads) {
-          const float x = lg[i];
-          if (x <= mid) ms += __expf((x - am.v) * inv_t);
-        }
-        ms = block_sum(ms, sm_f);
-        if (ms > target) hi = mid; else lo = mid;
-      }
-      thresh = lo;  // F(lo) <= target < F(hi): everything strictly above lo is in the nucleus
+    // optional per-row filters: keep_k[b] in [1, V) keeps the logits >= the k-th largest (ties kept), min_p[b] in (0, 1] keeps
+    // p >= min_p * p_max at temperature T, i.e. logit >= max + T * ln(min_p); a row with neither runs the plain path
+    const int kk = keep_k != nullptr ? keep_k[b] : 0;
+    const float mp = min_p != nullptr ? min_p[b] : 0.f;
+    const bool use_k = kk > 0 && kk < V;
+    if (use_k || mp > 0.f) {
+      __shared__ uint32_t sm_hist[kRadixBins];
+      __shared__ uint32_t sm_u[34];
+      const float kth = use_k ? radix_kth_largest(lg, V, kk, sm_hist, sm_u) : -INFINITY;
+      const float floor = mp > 0.f ? fmaxf(kth, am.v + temp * logf(mp)) : kth;
+      token = draw_token<true>(lg, V, am.v, temp, tp, kth, floor, seed, step, rng_row, sm_a, sm_f);
+    } else {
+      token = draw_token<false>(lg, V, am.v, temp, tp, -INFINITY, -INFINITY, seed, step, rng_row, sm_a, sm_f);
     }
-    // Gumbel-max over the kept set: argmax (logit / T + g), g = -log(-log(u))
-    ArgMax gm{-INFINITY, 0x7fffffff};
-    for (int i = threadIdx.x; i < V; i += kSampThreads) {
-      const float x = lg[i];
-      if (x > thresh) {
-        const float u = uniform01(seed, step, rng_row, i);
-        const float g = -__logf(-__logf(u));
-        gm = better(gm, ArgMax{(x - am.v) * inv_t + g, i});
-      }
-    }
-    gm = block_argmax(gm, sm_a);
-    token = gm.i;
   }
   if (threadIdx.x == 0) {
     tokens[b] = token;
@@ -183,14 +267,14 @@ cudaError_t apply_penalties_launch(float* logits, int B, int V, const int* rep_c
   return cudaGetLastError();
 }
 
-cudaError_t sample_launch(const float* logits, int B, int V, const float* temperature, const float* top_p,
-                          unsigned long long seed, unsigned long long step, const unsigned long long* row_rng, long long* tokens,
-                          float* logprobs, int top_k, long long* top_ids, float* top_lp, const void* tag_src, void* tag_dst,
-                          cudaStream_t s) {
+cudaError_t sample_launch(const float* logits, int B, int V, const float* temperature, const float* top_p, const int* keep_k,
+                          const float* min_p, unsigned long long seed, unsigned long long step, const unsigned long long* row_rng,
+                          long long* tokens, float* logprobs, int top_k, long long* top_ids, float* top_lp, const void* tag_src,
+                          void* tag_dst, cudaStream_t s) {
   if (B == 0) return cudaSuccess;
   if (top_k > 32) return cudaErrorInvalidValue;
-  (void)launch_pdl(sample_kernel, dim3(B), dim3(kSampThreads), 0, s, logits, V, temperature, top_p, seed, step, row_rng, tokens,
-                   logprobs, top_k, top_ids, top_lp, static_cast<const uint4*>(tag_src), static_cast<uint4*>(tag_dst));
+  (void)launch_pdl(sample_kernel, dim3(B), dim3(kSampThreads), 0, s, logits, V, temperature, top_p, keep_k, min_p, seed, step,
+                   row_rng, tokens, logprobs, top_k, top_ids, top_lp, static_cast<const uint4*>(tag_src), static_cast<uint4*>(tag_dst));
   return cudaGetLastError();
 }
 

@@ -255,12 +255,36 @@ def apply_penalties_(logits: torch.Tensor, rep_ctx: torch.Tensor, penalty: torch
     return logits
 
 
+def filter_keep(x: torch.Tensor, t: float, top_p: float, top_k: int, min_p: float) -> torch.Tensor:
+    """Kept set (bool ``[V]``) of one row at temperature ``t > 0``: top-k -> top-p -> min-p.
+
+    top-k keeps every logit >= the k-th largest (ties at the boundary kept; ``k <= 0`` or ``k >= V`` = off); top-p is the
+    nucleus of the top-k set renormalised at temperature ``t``; min-p keeps ``p >= min_p * p_max`` at temperature ``t``."""
+    V = x.shape[0]
+    keep = torch.ones(V, dtype=torch.bool, device=x.device)
+    if 0 < top_k < V:
+        kth = torch.sort(x, descending=True).values[top_k - 1]
+        keep &= x >= kth
+    if 0 < top_p < 1.0:
+        probs = torch.softmax((x / t).masked_fill(~keep, float("-inf")), dim=-1)
+        sp, si = torch.sort(probs, descending=False, stable=True)
+        nucleus = torch.zeros_like(keep)
+        nucleus[si] = torch.cumsum(sp, dim=0) > (1 - top_p)
+        keep &= nucleus
+    if min_p > 0:
+        probs = torch.softmax(x / t, dim=-1)
+        keep &= probs >= min_p * probs.max()
+    return keep
+
+
 def sample(logits: torch.Tensor, temperature: torch.Tensor, top_p: torch.Tensor,
-           generator: Optional[torch.Generator] = None, top_logprobs: int = 0):
+           generator: Optional[torch.Generator] = None, top_logprobs: int = 0,
+           top_k: Optional[torch.Tensor] = None, min_p: Optional[torch.Tensor] = None):
     """Batched sampler (reference shard/utils.py:126-139 + mlx_lm ``top_p_sampling``).
 
     ``logits`` fp32 ``[B, V]`` *after* bias / repetition penalty.  Per row: ``temp == 0`` -> argmax;
-    ``0 < top_p < 1`` -> nucleus; else categorical(softmax(logits / temp)).
+    ``0 < top_p < 1`` -> nucleus; else categorical(softmax(logits / temp)).  ``top_k`` (int ``[B]``, 0 = off) and ``min_p``
+    (float ``[B]``, 0 = off) optionally narrow the draw of a row with ``temp > 0`` (``filter_keep``).
     Returns ``(tokens int64 [B], token_logprob fp32 [B], topk_ids, topk_logprobs)`` where logprobs are
     ``logits - logsumexp(logits)`` (temperature **not** applied — reference utils.py:131)."""
     B, V = logits.shape
@@ -268,10 +292,17 @@ def sample(logits: torch.Tensor, temperature: torch.Tensor, top_p: torch.Tensor,
     logprobs = lf - torch.logsumexp(lf, dim=-1, keepdim=True)
     tokens = torch.empty(B, dtype=torch.int64, device=logits.device)
     t_cpu, p_cpu = temperature.tolist(), top_p.tolist()
+    k_cpu = top_k.tolist() if top_k is not None else [0] * B
+    m_cpu = min_p.tolist() if min_p is not None else [0.0] * B
     for b in range(B):
         t, p = t_cpu[b], p_cpu[b]
         if t == 0:
             tokens[b] = torch.argmax(lf[b])
+            continue
+        if 0 < k_cpu[b] < V or m_cpu[b] > 0:
+            keep = filter_keep(lf[b], t, p, int(k_cpu[b]), float(m_cpu[b]))
+            probs = torch.softmax((lf[b] / t).masked_fill(~keep, float("-inf")), dim=-1)
+            tokens[b] = torch.multinomial(probs, 1, generator=generator).squeeze()
             continue
         probs = torch.softmax(lf[b] / t, dim=-1)
         if 0 < p < 1.0:
@@ -291,7 +322,8 @@ def sample(logits: torch.Tensor, temperature: torch.Tensor, top_p: torch.Tensor,
 
 
 def sample_block(logits: torch.Tensor, sv, tag_out, toks_out, lp_out, top_ids_out, top_lp_out):
-    """Sampling driven by a step block (``parallel/graph_decode.py``): penalties, then per-sequence temperature / top-p with a
+    """Sampling driven by a step block (``parallel/graph_decode.py``): penalties, then per-sequence temperature / top-p (and the
+    optional top-k / min-p filters) with a
     per-request random stream — row ``b`` draws from a generator seeded with its ``(seed, tokens sampled so far)`` pair, so a
     request's tokens do not depend on which batch it decodes in.  Results go into the result-message views."""
     lf = logits.float().clone()
@@ -303,7 +335,8 @@ def sample_block(logits: torch.Tensor, sv, tag_out, toks_out, lp_out, top_ids_ou
     for b in range(B):
         g = torch.Generator(device=lf.device)
         g.manual_seed((rng[b][0] * 1000003 + rng[b][1] * 7919 + 12345) & 0x7FFFFFFFFFFFFFFF)
-        t, lp, ti, tl = sample(lf[b:b + 1], sv.temps[b:b + 1], sv.top_p[b:b + 1], generator=g, top_logprobs=k)
+        filt = dict(top_k=sv.keep_k[b:b + 1], min_p=sv.min_p[b:b + 1]) if sv.has_filter else {}
+        t, lp, ti, tl = sample(lf[b:b + 1], sv.temps[b:b + 1], sv.top_p[b:b + 1], generator=g, top_logprobs=k, **filt)
         toks_out[b], lp_out[b] = t[0], lp[0]
         if k:
             top_ids_out[b], top_lp_out[b] = ti[0], tl[0]

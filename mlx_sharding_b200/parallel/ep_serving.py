@@ -30,7 +30,7 @@ import torch
 import torch.distributed as dist
 
 from ..engine.core import LLMEngine, Request, StepInput
-from ..engine.sampler import SamplingParams
+from ..engine.sampler import SamplingParams, check_penalty_table
 from ..ops.meta import BatchMeta
 
 _SCRATCH_SEQ = -1
@@ -122,6 +122,7 @@ class LockstepGroup:
         assert self.rank == 0, "requests enter the group on rank 0"
         params = params or SamplingParams()
         params.validate()
+        check_penalty_table(params, max_tokens)
         if len(prompt) == 0:
             raise ValueError("empty prompt")
         if len(prompt) + max_tokens > self.engine.max_model_len:

@@ -7,7 +7,8 @@ for a given (group, batch size, block-table width, context bucket, sampling vari
 
 * defines the **step block** (``StepLayout``): ONE int32 vector that carries everything a stage needs for a step — a 16-byte
   step tag, the sampling block (per-sequence temperature / top-p / RNG state and, when any request uses them, repetition-penalty
-  contexts and logit-bias tables), the packed ``BatchMeta`` and the token ids.  Stage 0 builds it once per step; every stage
+  contexts, bias tables — logit_bias folded with presence / frequency penalties — and top-k / min-p filters), the packed
+  ``BatchMeta`` and the token ids.  Stage 0 builds it once per step; every stage
   copies it host->device with one pinned ``cudaMemcpyAsync``; in a multi-GPU pipeline it travels through the shared-memory
   launch ring (``shm_ring.py``);
 * defines the **result message** (``ResultLayout``): tag + sampled ids + their log-probs (+ top-k) in one buffer the last stage
@@ -27,6 +28,7 @@ from typing import Callable, Dict, List, Optional, Sequence, Tuple
 import numpy as np
 import torch
 
+from ..engine.sampler import bias_table
 from ..ops.meta import BatchMeta
 
 
@@ -48,26 +50,31 @@ def _pow2_at_least(n: int, lo: int) -> int:
 class StepLayout:
     """int32 word offsets of a step block for ``T`` tokens of ``B`` sequences.
 
-    ``C`` / ``NB`` > 0: the block carries repetition-penalty contexts ``[B, C]`` and logit-bias tables ``[B, NB]`` (only when a
-    request of the batch uses them); ``k`` = number of top log-probs the sampler returns (0 or 10)."""
+    ``C`` / ``NB`` > 0: the block carries repetition-penalty contexts ``[B, C]`` and additive bias tables ``[B, NB]`` (logit_bias
+    merged with the presence / frequency penalties; only when a request of the batch uses them); ``F`` = 1: it carries the
+    top-k / min-p filter section ``keep_k`` int32 ``[B]`` + ``min_p`` f32 ``[B]`` (only when a request of the batch filters its
+    draw); ``k`` = number of top log-probs the sampler returns (0 or 10)."""
 
-    __slots__ = ("T", "B", "mb", "C", "NB", "k", "tag", "temps", "top_p", "rng", "penalty", "rep", "bidx", "bval", "meta",
-                 "tokens", "size")
+    __slots__ = ("T", "B", "mb", "C", "NB", "k", "F", "tag", "temps", "top_p", "rng", "penalty", "rep", "bidx", "bval", "keep_k",
+                 "min_p", "meta", "tokens", "size")
 
-    def __init__(self, T: int, B: int, mb: int, C: int = 0, NB: int = 0, k: int = 0):
-        self.T, self.B, self.mb, self.C, self.NB, self.k = T, B, mb, C, NB, k
+    def __init__(self, T: int, B: int, mb: int, C: int = 0, NB: int = 0, k: int = 0, F: int = 0):
+        self.T, self.B, self.mb, self.C, self.NB, self.k, self.F = T, B, mb, C, NB, k, F
         o = 0
         self.tag = o; o += 4                       # [seq_lo, seq_hi, k, flags] — 16 bytes, copied into the result message
         self.temps = o; o += B
         self.top_p = o; o += B
         o = (o + 1) // 2 * 2
         self.rng = o; o += 4 * B                   # int64 [B, 2] = (seed, tokens sampled so far) per sequence
-        self.penalty = self.rep = self.bidx = self.bval = -1
+        self.penalty = self.rep = self.bidx = self.bval = self.keep_k = self.min_p = -1
         if C or NB:
             self.penalty = o; o += B
             self.rep = o; o += B * C
             self.bidx = o; o += B * NB
             self.bval = o; o += B * NB
+        if F:
+            self.keep_k = o; o += B
+            self.min_p = o; o += B
         o = (o + 3) // 4 * 4
         self.meta = o; o += BatchMeta.packed_size(T, B, mb)
         o = (o + 1) // 2 * 2
@@ -75,11 +82,11 @@ class StepLayout:
         self.size = (o + 3) // 4 * 4
 
     @property
-    def key(self) -> Tuple[int, int, int, int, int, int]:
-        return (self.T, self.B, self.mb, self.C, self.NB, self.k)
+    def key(self) -> Tuple[int, int, int, int, int, int, int]:
+        return (self.T, self.B, self.mb, self.C, self.NB, self.k, self.F)
 
 
-HEADER_WORDS = 8      # prepended to the block on the wire: T, B, mb, C, NB, k, is_prefill, 0
+HEADER_WORDS = 8      # prepended to the block on the wire: T, B, mb, C, NB, k, is_prefill, F (filter section present)
 
 
 class ResultLayout:
@@ -114,14 +121,17 @@ class ResultLayout:
         return tag, toks, lp, ti, tl
 
 
-def sampling_variant(params) -> Tuple[int, int, int]:
-    """(C, NB, k) table sizes a batch needs: 0/0 when no request uses a repetition penalty or logit bias."""
+def sampling_variant(params, counts=None) -> Tuple[int, int, int]:
+    """(C, NB, k) table sizes a batch needs: 0/0 when no request uses a repetition penalty, logit bias or (once it has generated
+    a token) a presence / frequency penalty.  ``counts[b]``: the ``OutputCounts`` of requests with such a penalty."""
     C = NB = k = 0
-    for p in params:
+    for b, p in enumerate(params):
         if p.repetition_penalty not in (0, 1.0) and p.repetition_context_size > 0:
             C = max(C, int(p.repetition_context_size))
-        if p.logit_bias:
-            NB = max(NB, len(p.logit_bias))
+        nb = len(p.logit_bias) if p.logit_bias else 0
+        if counts is not None and counts[b]:
+            nb += len(counts[b])        # upper bound of the merged table (entries for the same id are folded into one)
+        NB = max(NB, nb)
         if p.logprobs:
             k = 10
     if C or NB:
@@ -136,10 +146,8 @@ def decode_bucket(B: int) -> int:
     return (B + 7) // 8 * 8 if B <= 64 else (B + 15) // 16 * 16
 
 
-def _pad_decode(meta: BatchMeta, tokens: torch.Tensor, params, contexts, rng, Bp: int):
+def _pad_decode(meta: BatchMeta, tokens: torch.Tensor, params, contexts, rng, counts, Bp: int):
     """Pad a pure-decode step to ``Bp`` sequences with dummy rows that read / write the reserved null page (page 0, position 0)."""
-    from ..engine.sampler import SamplingParams
-
     B, n = meta.num_seqs, Bp - meta.num_seqs
     z = lambda k: torch.zeros(k, dtype=torch.int32)
     mb = meta.block_tables.shape[1]
@@ -151,15 +159,18 @@ def _pad_decode(meta: BatchMeta, tokens: torch.Tensor, params, contexts, rng, Bp
     params = list(params) + [_PAD_PARAMS] * n
     contexts = (list(contexts) + [[]] * n) if contexts is not None else None
     rng = (list(rng) + [(0, 0)] * n) if rng is not None else None
-    return meta, tokens, params, contexts, rng
+    counts = (list(counts) + [None] * n) if counts is not None else None
+    return meta, tokens, params, contexts, rng, counts
 
 
 _PAD_PARAMS = None
 
 
 def pack_step(seq: int, meta: BatchMeta, tokens: torch.Tensor, params, contexts, rng, is_prefill: bool,
-              pad_decode: bool = False) -> Tuple[np.ndarray, StepLayout]:
-    """Host side (stage 0): one int32 vector ``[header | step block]`` for this step.  ``rng[b]`` = (seed, sampled so far).
+              pad_decode: bool = False, counts=None) -> Tuple[np.ndarray, StepLayout]:
+    """Host side (stage 0): one int32 vector ``[header | step block]`` for this step.  ``rng[b]`` = (seed, sampled so far);
+    ``counts[b]`` = ``OutputCounts`` of a request with a presence / frequency penalty (else ``None``), folded with
+    its ``logit_bias`` into one bias entry per token id.
 
     ``pad_decode``: a pure decode step is padded to the next batch-size bucket (``decode_bucket``) with dummy rows on the null
     page, so that continuous batching — sequences joining and leaving every few steps — keeps replaying a handful of captured
@@ -172,13 +183,14 @@ def pack_step(seq: int, meta: BatchMeta, tokens: torch.Tensor, params, contexts,
                 from ..engine.sampler import SamplingParams
 
                 _PAD_PARAMS = SamplingParams()
-            meta, tokens, params, contexts, rng = _pad_decode(meta, tokens, params, contexts, rng, Bp)
+            meta, tokens, params, contexts, rng, counts = _pad_decode(meta, tokens, params, contexts, rng, counts, Bp)
     T, B = meta.num_tokens, meta.num_seqs
     mb = meta.block_tables.shape[1]
-    C, NB, k = sampling_variant(params)
-    lay = StepLayout(T, B, mb, C, NB, k)
+    C, NB, k = sampling_variant(params, counts)
+    F = int(any(p.uses_filter for p in params))
+    lay = StepLayout(T, B, mb, C, NB, k, F)
     buf = np.zeros(HEADER_WORDS + lay.size, dtype=np.int32)
-    buf[:HEADER_WORDS] = (T, B, mb, C, NB, k, int(is_prefill), 0)
+    buf[:HEADER_WORDS] = (T, B, mb, C, NB, k, int(is_prefill), F)
     blk = buf[HEADER_WORDS:]
     blk[lay.tag] = seq & 0x7FFFFFFF
     blk[lay.tag + 1] = (seq >> 31) & 0x7FFFFFFF
@@ -202,16 +214,20 @@ def pack_step(seq: int, meta: BatchMeta, tokens: torch.Tensor, params, contexts,
                 if c:
                     rep[b, :len(c)] = c
                 pen[b] = p.repetition_penalty
-            for j, (tid, v) in enumerate((p.logit_bias or {}).items()):
-                bidx[b, j], bval[b, j] = int(tid), float(v)
+            ids, vals = bias_table(p, counts[b] if counts is not None else None)
+            bidx[b, :len(ids)] = ids
+            bval[b, :len(ids)] = vals
+    if F:
+        blk[lay.keep_k:lay.keep_k + B] = [max(p.top_k, 0) if p.uses_filter else 0 for p in params]
+        f32[lay.min_p:lay.min_p + B] = [p.min_p if p.uses_filter else 0.0 for p in params]
     blk[lay.meta:lay.meta + BatchMeta.packed_size(T, B, mb)] = meta.pack().numpy()
     blk[lay.tokens:lay.tokens + 2 * T].view(np.int64)[:] = tokens.numpy()
     return buf, lay
 
 
 def unpack_header(buf: np.ndarray) -> Tuple[StepLayout, bool]:
-    T, B, mb, C, NB, k, pre, _ = (int(v) for v in buf[:HEADER_WORDS])
-    return StepLayout(T, B, mb, C, NB, k), bool(pre)
+    T, B, mb, C, NB, k, pre, F = (int(v) for v in buf[:HEADER_WORDS])
+    return StepLayout(T, B, mb, C, NB, k, F), bool(pre)
 
 
 class StepViews:
@@ -231,6 +247,9 @@ class StepViews:
             self.rep = flat[lay.rep:lay.rep + B * lay.C].view(B, lay.C)
             self.bidx = flat[lay.bidx:lay.bidx + B * lay.NB].view(B, lay.NB)
             self.bval = f32[lay.bval:lay.bval + B * lay.NB].view(B, lay.NB)
+        self.has_filter = bool(lay.F)
+        self.keep_k = flat[lay.keep_k:lay.keep_k + B] if lay.F else None
+        self.min_p = f32[lay.min_p:lay.min_p + B] if lay.F else None
         o = lay.meta + 6
         take = lambda n: (flat[o:o + n], o + n)
         pos, o = take(T)

@@ -104,6 +104,18 @@ def parse_request_params(body: dict) -> dict:
         raise RequestError("model must be a string")
     if p["seed"] is not None and (not isinstance(p["seed"], int) or isinstance(p["seed"], bool)):
         raise RequestError("seed must be an integer")
+    # OpenAI's presence / frequency penalties and the top_k / min_p filters of vLLM, llama.cpp and mlx_lm (null = default)
+    num = lambda v: isinstance(v, (float, int)) and not isinstance(v, bool)
+    for name, default in (("top_k", 0), ("min_p", 0.0), ("presence_penalty", 0.0), ("frequency_penalty", 0.0)):
+        v = body.get(name)
+        p[name] = default if v is None else v
+    if not isinstance(p["top_k"], int) or isinstance(p["top_k"], bool) or p["top_k"] < -1:
+        raise RequestError("top_k must be an integer >= -1 (0 or -1 disables it)")
+    if not num(p["min_p"]) or not 0 <= p["min_p"] <= 1:
+        raise RequestError("min_p must be a float between 0 and 1")
+    for name in ("presence_penalty", "frequency_penalty"):
+        if not num(p[name]) or not -2 <= p[name] <= 2:
+            raise RequestError(f"{name} must be a float between -2 and 2")
     return p
 
 
@@ -375,7 +387,10 @@ class APIHandler(BaseHTTPRequestHandler):
             params = SamplingParams(temperature=float(prm["temperature"]), top_p=float(prm["top_p"]),
                                     repetition_penalty=float(prm["repetition_penalty"]),
                                     repetition_context_size=prm["repetition_context_size"],
-                                    logit_bias=prm["logit_bias"], logprobs=max(prm["logprobs"], 0), seed=prm["seed"])
+                                    logit_bias=prm["logit_bias"], logprobs=max(prm["logprobs"], 0), seed=prm["seed"],
+                                    top_k=prm["top_k"], min_p=float(prm["min_p"]),
+                                    presence_penalty=float(prm["presence_penalty"]),
+                                    frequency_penalty=float(prm["frequency_penalty"]))
             req = self.engine.submit(prompt, params, max_tokens=prm["max_tokens"],
                                      eos_token_id=self.tokenizer.eos_token_id, stop_id_sequences=stop_ids)
         except (RequestError, ValueError, AssertionError, KeyError) as e:
