@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """Sampler microbenchmark: ``sample_into`` (ops/csrc/sampler.cu) on B rows (default 64) of V = 102400 seeded fp32 logits, CUDA-event
-timed, for the default path and the top-p / top-k / min-p filters.  Prints microseconds per call with the card name and power
-limit, one JSON line at the end.
+timed, for the default path, the top-p / top-k / min-p filters and token masks (structured output) with about 1 % and 50 % of
+the ids allowed.  Prints microseconds per call with the card name and power limit, one JSON line at the end.
 
 ``--dump DIR`` writes the default-path tokens and log-probs at T = 0, T = 1 and T = 1 with top-p 0.9 (``default_*.npy``).  That
 part passes only the arguments every build's ``sample_into`` has, so the dumps of two builds can be compared byte for byte."""
@@ -56,17 +56,29 @@ def main():
             np.save(os.path.join(a.dump, f"default_{name}_tokens.npy"), toks.cpu().numpy())
             np.save(os.path.join(a.dump, f"default_{name}_logprobs.npy"), lp.cpu().numpy())
 
-    cases = [("greedy", 0.0, 1.0, 0, 0.0), ("T=1", 1.0, 1.0, 0, 0.0), ("top-p 0.9", 1.0, 0.9, 0, 0.0),
-             ("top-k 50", 1.0, 1.0, 50, 0.0), ("top-k 50 + top-p 0.9", 1.0, 0.9, 50, 0.0), ("min-p 0.05", 1.0, 1.0, 0, 0.05)]
+    # token masks: each bit set with probability ~1 % / ~50 % (seeded), int32 [B, ceil(V/32)]
+    gm = torch.Generator(device=dev).manual_seed(1)
+    words = (V + 31) // 32
+    bits = lambda frac: (torch.rand(B, words * 32, device=dev, generator=gm) < frac).view(B, words, 32).to(torch.int64)
+    pack = lambda b: (b << torch.arange(32, device=dev)).sum(-1).to(torch.int32).contiguous()   # wraps bit 31 into the sign
+    masks = {"1%": pack(bits(0.01)), "50%": pack(bits(0.5))}
+    cases = [("greedy", 0.0, 1.0, 0, 0.0, None), ("T=1", 1.0, 1.0, 0, 0.0, None), ("top-p 0.9", 1.0, 0.9, 0, 0.0, None),
+             ("top-k 50", 1.0, 1.0, 50, 0.0, None), ("top-k 50 + top-p 0.9", 1.0, 0.9, 50, 0.0, None),
+             ("min-p 0.05", 1.0, 1.0, 0, 0.05, None)]
+    for m in ("1%", "50%"):
+        cases += [(f"mask {m}, greedy", 0.0, 1.0, 0, 0.0, m), (f"mask {m}, T=1", 1.0, 1.0, 0, 0.0, m),
+                  (f"mask {m}, top-p 0.9", 1.0, 0.9, 0, 0.0, m)]
     info = card()
     print(f"sample_into, B={B}, V={V}, fp32 logits; {info['gpu']}, power limit {info['power_limit']}")
     rows = []
-    for name, t, p, k, mp in cases:
+    for name, t, p, k, mp, m in cases:
         args = (logits, full(t), full(p), rng, 0, toks, lp)
         kw = dict(keep_k=full(k, torch.int32), min_p=full(mp)) if (k or mp) else {}
+        if m is not None:
+            kw["allow"] = masks[m]
         try:
             C.sample_into(*args, **kw)
-        except TypeError:          # a build without the filter arguments
+        except TypeError:          # a build without the filter / mask arguments
             print(f"  {name:<24} not supported by this build")
             rows.append({"case": name, "us": None})
             continue

@@ -19,6 +19,7 @@ import time
 from dataclasses import dataclass, field
 from typing import Dict, List, Optional, Sequence
 
+import numpy as np
 import torch
 
 from ..ops.meta import BatchMeta
@@ -43,6 +44,9 @@ class StepInput:
     # per sequence: output token counts of requests with a presence / frequency penalty (else None); None when no
     # request of the engine uses one
     counts: Optional[List[Optional[OutputCounts]]] = None
+    # token masks int32 [B, ceil(V/32)] when a sampled row of this step belongs to a request with a response_format (the other
+    # rows all ones), else None
+    allow: Optional[np.ndarray] = None
 
 
 @dataclass
@@ -76,6 +80,7 @@ class Request:
         self.output: List[int] = []
         # times each token id occurs in ``output``: kept only for the presence / frequency penalties
         self.counts: Optional[OutputCounts] = OutputCounts() if params.uses_output_penalty else None
+        self.matcher = None           # grammar matcher of a request with a response_format (engine/grammar.py)
         self.events: "queue.SimpleQueue[TokenEvent]" = queue.SimpleQueue()   # C implementation: one put per generated token
         self.finished = False
         self.finish_reason: Optional[str] = None
@@ -147,6 +152,10 @@ class LLMEngine:
         self.stats = dict(steps=0, prefill_tokens=0, decode_tokens=0, finished=0, prefix_cached_tokens=0)
         self.sinks: list = []      # event sinks of the API worker processes (server/frontend.py): flushed once per scheduler iteration
         self._penalised = 0        # running requests with a presence / frequency penalty (their steps carry output counts)
+        # structured output (engine/grammar.py::GrammarBackend, set by the server next to the tokenizer); None = response_format
+        # is refused
+        self.grammar = None
+        self._constrained = 0      # running requests with a response_format (their steps carry token masks)
 
     # -------------------------------------------------------------------------- public API
     def submit(self, prompt: Sequence[int], params: Optional[SamplingParams] = None, max_tokens: int = 100,
@@ -161,7 +170,14 @@ class LLMEngine:
         if len(prompt) + max_tokens > self.max_model_len:
             raise ValueError(f"prompt ({len(prompt)}) + max_tokens ({max_tokens}) exceeds max_model_len "
                              f"({self.max_model_len})")
+        matcher = None
+        if params.response_format is not None:
+            if self.grammar is None:
+                raise ValueError("response_format is not available on this server (structured output needs the xgrammar "
+                                 "package and a tokenizer on the engine)")
+            matcher = self.grammar.matcher(params.response_format)   # ValueError: the schema does not compile
         r = Request(prompt, params, max_tokens, eos_token_id, stop_id_sequences)
+        r.matcher = matcher
         if events is not None:
             r.events = events
             events.req = r
@@ -250,6 +266,7 @@ class LLMEngine:
                 r.events.put(None)
             self.groups[g] = []
         self._penalised = 0
+        self._constrained = 0
         for s in self.sinks:
             s.flush()
 
@@ -289,6 +306,8 @@ class LLMEngine:
             self.groups[g].append(r)
             if r.counts is not None:
                 self._penalised += 1
+            if r.matcher is not None:
+                self._constrained += 1
 
     def _build_step(self, g: int) -> Optional[StepInput]:
         reqs = [r for r in self.groups[g] if not r.finished]
@@ -333,9 +352,27 @@ class LLMEngine:
         ctxs = [(r.prompt + r.output)[-max(1, r.params.repetition_context_size):]
                 if r.params.repetition_penalty not in (0, 1.0) else [] for r in seqs]
         counts = [r.counts for r in seqs] if self._penalised else None
+        allow = self._token_masks(seqs, mask) if self._constrained else None
         return StepInput(g, [r.id for r in seqs], torch.tensor(toks, dtype=torch.int64), meta,
                          [r.params for r in seqs], ctxs, mask, is_prefill, [(r.seed, len(r.output)) for r in seqs],
-                         counts), seqs, q_lens
+                         counts, allow), seqs, q_lens
+
+    def _token_masks(self, seqs: List[Request], mask: List[bool]) -> Optional[np.ndarray]:
+        """Token masks of a step: the grammar's next-token masks of the constrained requests that sample in it (one batched
+        fill), all ones for every other row; ``None`` when no constrained request samples."""
+        rows = [b for b, r in enumerate(seqs) if mask[b] and r.matcher is not None]
+        if not rows:
+            return None
+        allow = np.full((len(seqs), self.grammar.words), -1, dtype=np.int32)
+        self.grammar.fill([seqs[b].matcher for b in rows], allow, rows)
+        return allow
+
+    def _accept_tokens(self, seqs: List[Request], inp: StepInput, out: StepOutput) -> Dict[int, bool]:
+        """Feed the sampled tokens of the constrained requests to their matchers (one batched call): row -> accepted."""
+        rows = [b for b, r in enumerate(seqs) if r.matcher is not None and inp.sample_mask[b] and not r.cancelled]
+        if not rows:
+            return {}
+        return dict(zip(rows, self.grammar.accept([seqs[b].matcher for b in rows], [int(out.tokens[b]) for b in rows])))
 
     def _finish(self, r: Request, reason: str):
         r.finished, r.finish_reason = True, reason
@@ -344,9 +381,18 @@ class LLMEngine:
         self.stats["finished"] += 1
         if r.counts is not None:
             self._penalised -= 1
+        if r.matcher is not None:
+            self._constrained -= 1
+
+    def _fail(self, r: Request, e: BaseException):
+        """Fail one running request (its handler raises ``e``: HTTP 500 or an SSE error); the rest of the batch carries on."""
+        self._finish(r, "error")
+        r.error = e
+        r.events.put(None)
 
     def _process(self, g: int, seqs: List[Request], q_lens: List[int], inp: StepInput, out: StepOutput):
         length, n_decode = self.table.length, 0
+        fits = self._accept_tokens(seqs, inp, out) if self._constrained else None
         for b, r in enumerate(seqs):
             if inp.is_prefill and r.prefilled < len(r.prompt):
                 r.prefilled += q_lens[b]
@@ -363,6 +409,11 @@ class LLMEngine:
             if not inp.sample_mask[b]:
                 continue
             tok = int(out.tokens[b])
+            if r.matcher is not None and not fits[b]:
+                # the sampler draws only allowed ids, so this is a row without any allowed id of finite logit: the token never
+                # reaches the client
+                self._fail(r, RuntimeError(f"sampled token {tok} does not fit the request's response_format"))
+                continue
             if r.t_first is None:
                 r.t_first = time.perf_counter()
             r.output.append(tok)

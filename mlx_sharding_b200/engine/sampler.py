@@ -33,6 +33,9 @@ class SamplingParams:
     # logit[j] -= frequency_penalty * count[j] + presence_penalty * (count[j] > 0)
     presence_penalty: float = 0.0
     frequency_penalty: float = 0.0
+    # structured output: canonical JSON text of the request's OpenAI ``response_format`` (``engine/grammar.py::canonical_format``);
+    # None = unconstrained
+    response_format: Optional[str] = None
 
     def validate(self):
         if self.temperature < 0:
@@ -53,6 +56,10 @@ class SamplingParams:
             raise ValueError("presence_penalty must be a float between -2 and 2")
         if not (-2 <= self.frequency_penalty <= 2):
             raise ValueError("frequency_penalty must be a float between -2 and 2")
+        if self.response_format is not None:
+            from .grammar import check_format_text
+
+            check_format_text(self.response_format)
 
     @property
     def uses_filter(self) -> bool:
@@ -163,9 +170,10 @@ class Sampler:
 
     def __call__(self, logits: torch.Tensor, params: List[SamplingParams],
                  contexts: Optional[List[List[int]]] = None,
-                 counts: Optional[List[Optional[OutputCounts]]] = None) -> SampleOutput:
+                 counts: Optional[List[Optional[OutputCounts]]] = None, allow=None) -> SampleOutput:
         """``logits`` fp32 ``[B, V]``; ``contexts[b]`` = recent token ids for the repetition penalty; ``counts[b]`` = how often
-        each token id has been generated by that request (presence / frequency penalties)."""
+        each token id has been generated by that request (presence / frequency penalties); ``allow`` = token masks int32
+        ``[B, ceil(V/32)]`` of structured-output requests (rows of the others all ones), or ``None``."""
         B = logits.shape[0]
         assert len(params) == B
         logits = logits.float()
@@ -199,5 +207,7 @@ class Sampler:
         if any(p.uses_filter for p in params):
             filt = dict(top_k=torch.tensor([max(p.top_k, 0) for p in params], dtype=torch.int32, device=self.device),
                         min_p=torch.tensor([p.min_p for p in params], dtype=torch.float32, device=self.device))
+        if allow is not None:
+            filt["allow"] = torch.as_tensor(allow, dtype=torch.int32).to(self.device)
         toks, lp, ti, tl = self.ops.sample(logits, temps, top_p, generator=self.gen, top_logprobs=k, **filt)
         return SampleOutput(toks, lp, ti, tl)

@@ -388,12 +388,13 @@ _step = [0]
 
 
 def sample(logits, temperature, top_p, generator: Optional[torch.Generator] = None, top_logprobs: int = 0,
-           top_k: Optional[torch.Tensor] = None, min_p: Optional[torch.Tensor] = None):
-    """``top_k`` (int32 ``[B]``, 0 = off) / ``min_p`` (fp32 ``[B]``, 0 = off): optional per-row filters of the temperature draw."""
+           top_k: Optional[torch.Tensor] = None, min_p: Optional[torch.Tensor] = None, allow: Optional[torch.Tensor] = None):
+    """``top_k`` (int32 ``[B]``, 0 = off) / ``min_p`` (fp32 ``[B]``, 0 = off): optional per-row filters of the temperature draw;
+    ``allow`` (int32 ``[B, ceil(V/32)]``): optional token mask of the draw (bit ``j & 31`` of word ``j >> 5`` = id ``j`` allowed)."""
     seed = generator.initial_seed() if generator is not None else 0
     _step[0] += 1
     toks, lp, ti, tl = C().sample(logits.contiguous(), temperature, top_p, int(seed) & 0x7FFFFFFFFFFFFFFF, _step[0],
-                                  int(top_logprobs), top_k, min_p)
+                                  int(top_logprobs), top_k, min_p, None if allow is None else allow.contiguous())
     if top_logprobs > 0:
         return toks, lp, ti, tl
     return toks, lp, None, None
@@ -416,14 +417,14 @@ def mla_decode(q, pool, meta: BatchMeta, scale: float, nsplit: int = 0):
 
 def sample_block(logits, sv, tag_out, toks_out, lp_out, top_ids_out, top_lp_out):
     """Sampling driven by a step block in device memory (``parallel/graph_decode.py``): every per-step input — temperatures,
-    nucleus thresholds, per-request (seed, step) RNG state, penalty contexts, bias tables, top-k / min-p filters, the step tag —
-    is read by the kernels from the block, so the same captured CUDA graph serves greedy and sampled requests."""
+    nucleus thresholds, per-request (seed, step) RNG state, penalty contexts, bias tables, top-k / min-p filters, token masks,
+    the step tag — is read by the kernels from the block, so the same captured CUDA graph serves greedy and sampled requests."""
     logits = logits.contiguous()
     if sv.has_pen:
         C().apply_penalties_(logits, sv.rep, sv.penalty, sv.bidx, sv.bval)
     k = 0 if top_ids_out is None else int(top_ids_out.shape[1])
     C().sample_into(logits, sv.temps, sv.top_p, sv.rng, k, toks_out, lp_out, top_ids_out, top_lp_out, sv.tag, tag_out,
-                    sv.keep_k, sv.min_p)
+                    sv.keep_k, sv.min_p, sv.allow)
 
 
 def mla_rope_kv_write(q, k_pe, kv, kpool, vpool, meta: BatchMeta, spec: RopeSpec, nope: int, vdim: int):

@@ -576,9 +576,18 @@ static const float* min_p_ptr(const c10::optional<Tensor>& min_p, const Tensor& 
               min_p->numel() >= logits.size(0), "min_p must be a contiguous float32 [B] tensor on the logits' device");
   return min_p->data_ptr<float>();
 }
+// optional token mask of a structured-output batch: int32 [B, ceil(V/32)], bit j & 31 of word j >> 5 = "id j may be drawn"
+static const uint32_t* allow_ptr(const c10::optional<Tensor>& allow, const Tensor& logits) {
+  if (!allow.has_value()) return nullptr;
+  TORCH_CHECK(allow->scalar_type() == torch::kInt32 && allow->is_contiguous() && allow->device() == logits.device() &&
+              allow->dim() == 2 && allow->size(0) == logits.size(0) && allow->size(1) == (logits.size(1) + 31) / 32,
+              "allow must be a contiguous int32 [B, ceil(V/32)] tensor on the logits' device");
+  return reinterpret_cast<const uint32_t*>(allow->data_ptr<int>());
+}
 
 std::vector<Tensor> sample(const Tensor& logits, const Tensor& temperature, const Tensor& top_p, int64_t seed, int64_t step, int64_t top_k,
-                           const c10::optional<Tensor>& keep_k, const c10::optional<Tensor>& min_p) {
+                           const c10::optional<Tensor>& keep_k, const c10::optional<Tensor>& min_p,
+                           const c10::optional<Tensor>& allow) {
   TORCH_CHECK(logits.is_cuda() && logits.scalar_type() == torch::kFloat32 && logits.is_contiguous());
   const c10::cuda::CUDAGuard guard(logits.device());
   const int B = (int)logits.size(0);
@@ -588,7 +597,7 @@ std::vector<Tensor> sample(const Tensor& logits, const Tensor& temperature, cons
   Tensor top_ids = torch::empty({B, top_k}, torch::dtype(torch::kInt64).device(dev));
   Tensor top_lp = torch::empty({B, top_k}, torch::dtype(torch::kFloat32).device(dev));
   LAUNCH_OK(b200::sample_launch(logits.data_ptr<float>(), B, (int)logits.size(1), temperature.data_ptr<float>(), top_p.data_ptr<float>(),
-                              keep_k_ptr(keep_k, logits), min_p_ptr(min_p, logits), (unsigned long long)seed, (unsigned long long)step, nullptr, reinterpret_cast<long long*>(tokens.data_ptr<int64_t>()),
+                              keep_k_ptr(keep_k, logits), min_p_ptr(min_p, logits), allow_ptr(allow, logits), (unsigned long long)seed, (unsigned long long)step, nullptr, reinterpret_cast<long long*>(tokens.data_ptr<int64_t>()),
                               lp.data_ptr<float>(), (int)top_k, reinterpret_cast<long long*>(top_ids.data_ptr<int64_t>()),
                               top_lp.data_ptr<float>(), nullptr, nullptr, cur_stream()));
   return {tokens, lp, top_ids, top_lp};
@@ -599,7 +608,7 @@ std::vector<Tensor> sample(const Tensor& logits, const Tensor& temperature, cons
 void sample_into(const Tensor& logits, const Tensor& temperature, const Tensor& top_p, const Tensor& row_rng, int64_t top_k,
                  Tensor tokens, Tensor lp, const c10::optional<Tensor>& top_ids, const c10::optional<Tensor>& top_lp,
                  const c10::optional<Tensor>& tag_src, const c10::optional<Tensor>& tag_dst, const c10::optional<Tensor>& keep_k,
-                 const c10::optional<Tensor>& min_p) {
+                 const c10::optional<Tensor>& min_p, const c10::optional<Tensor>& allow) {
   TORCH_CHECK(logits.is_cuda() && logits.scalar_type() == torch::kFloat32 && logits.is_contiguous());
   TORCH_CHECK(row_rng.scalar_type() == torch::kInt64 && row_rng.is_contiguous() && row_rng.numel() >= 2 * logits.size(0));
   TORCH_CHECK(tokens.scalar_type() == torch::kInt64 && lp.scalar_type() == torch::kFloat32);
@@ -610,7 +619,7 @@ void sample_into(const Tensor& logits, const Tensor& temperature, const Tensor& 
                 reinterpret_cast<uintptr_t>(tag_src->data_ptr()) % 16 == 0 && reinterpret_cast<uintptr_t>(tag_dst->data_ptr()) % 16 == 0);
   const c10::cuda::CUDAGuard guard(logits.device());
   LAUNCH_OK(b200::sample_launch(logits.data_ptr<float>(), (int)logits.size(0), (int)logits.size(1), temperature.data_ptr<float>(),
-                              top_p.data_ptr<float>(), keep_k_ptr(keep_k, logits), min_p_ptr(min_p, logits), 0ull, 0ull, reinterpret_cast<const unsigned long long*>(row_rng.data_ptr<int64_t>()),
+                              top_p.data_ptr<float>(), keep_k_ptr(keep_k, logits), min_p_ptr(min_p, logits), allow_ptr(allow, logits), 0ull, 0ull, reinterpret_cast<const unsigned long long*>(row_rng.data_ptr<int64_t>()),
                               reinterpret_cast<long long*>(tokens.data_ptr<int64_t>()), lp.data_ptr<float>(), (int)top_k,
                               top_k ? reinterpret_cast<long long*>(top_ids->data_ptr<int64_t>()) : nullptr,
                               top_k ? top_lp->data_ptr<float>() : nullptr, tag_src.has_value() ? tag_src->data_ptr() : nullptr,
@@ -838,11 +847,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("zero_counts") = py::none(), py::arg("norm_w") = py::none(), py::arg("norm_eps") = 1e-6, py::arg("normed") = py::none());
   m.def("apply_penalties_", &apply_penalties_);
   m.def("sample", &sample, py::arg("logits"), py::arg("temperature"), py::arg("top_p"), py::arg("seed"), py::arg("step"),
-        py::arg("top_k"), py::arg("keep_k") = py::none(), py::arg("min_p") = py::none());
+        py::arg("top_k"), py::arg("keep_k") = py::none(), py::arg("min_p") = py::none(), py::arg("allow") = py::none());
   m.def("sample_into", &sample_into, py::arg("logits"), py::arg("temperature"), py::arg("top_p"), py::arg("row_rng"), py::arg("top_k"),
         py::arg("tokens"), py::arg("logprobs"), py::arg("top_ids") = py::none(), py::arg("top_lp") = py::none(),
         py::arg("tag_src") = py::none(), py::arg("tag_dst") = py::none(), py::arg("keep_k") = py::none(),
-        py::arg("min_p") = py::none());
+        py::arg("min_p") = py::none(), py::arg("allow") = py::none());
   m.def("ipc_alloc", &ipc_alloc);
   m.def("ipc_open", &ipc_open);
   m.def("enable_peer_access", &enable_peer_access);

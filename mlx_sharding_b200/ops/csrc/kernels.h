@@ -113,10 +113,12 @@ cudaError_t apply_penalties_launch(float* logits, int B, int V, const int* rep_c
 // tag_src/tag_dst (optional): 16 bytes copied verbatim next to the results (scheduler step id)
 // keep_k / min_p (optional, device, [B]): per-row top-k (0 or >= V = off) and min-p (0 = off) filters of the temperature draw;
 // a null pointer or an off value leaves the row on the plain top-p / categorical path
+// allow (optional, device, [B, ceil(V/32)] words): token j of row b may be drawn iff bit j & 31 of allow[b][j >> 5] is set; the
+// reported log-probs ignore it, and a row with no allowed id of finite logit is sampled unmasked
 cudaError_t sample_launch(const float* logits, int B, int V, const float* temperature, const float* top_p, const int* keep_k,
-                          const float* min_p, unsigned long long seed, unsigned long long step, const unsigned long long* row_rng,
-                          long long* tokens, float* logprobs, int top_k, long long* top_ids, float* top_lp, const void* tag_src,
-                          void* tag_dst, cudaStream_t s);
+                          const float* min_p, const uint32_t* allow, unsigned long long seed, unsigned long long step,
+                          const unsigned long long* row_rng, long long* tokens, float* logprobs, int top_k, long long* top_ids,
+                          float* top_lp, const void* tag_src, void* tag_dst, cudaStream_t s);
 
 // ---- p2p.cu
 cudaError_t wait_flag_launch(const uint32_t* flag, uint32_t expected, uint32_t* error_flag, cudaStream_t s);

@@ -8,6 +8,8 @@
 // Optional per-row filters, in the order top-k -> top-p -> min-p: top-k keeps the logits >= the exact k-th largest (radix select,
 // ties kept) and restricts the nucleus to that set; min-p is one logit threshold.  Presence / frequency penalties arrive folded
 // into the additive bias table of apply_penalties_kernel.
+// Optional token mask (structured output): one bit per vocabulary id; disallowed ids read as -inf everywhere the draw looks (greedy
+// argmax, the temperature anchor, top-k, top-p sums, min-p, Gumbel) while the reported log-probs keep the full row.
 #include "kernels.h"
 #include "launch.h"
 #include "ptx.cuh"
@@ -68,12 +70,25 @@ __device__ __forceinline__ float key_value(uint32_t k) {
   return __uint_as_float((k & 0x80000000u) ? (k & 0x7fffffffu) : ~k);
 }
 
+// Logit of id i as the draw sees it: -inf when the row has a mask (`al` != nullptr) and bit i & 31 of al[i >> 5] is clear.  The
+// 32 ids a warp reads in one iteration share one mask word, so the mask costs one broadcast load per warp and pass.
+template <bool kMask>
+__device__ __forceinline__ float draw_logit(const float* __restrict__ lg, const uint32_t* __restrict__ al, int i) {
+  const float x = lg[i];
+  if constexpr (kMask) {
+    if (al != nullptr && !((al[i >> 5] >> (i & 31)) & 1u)) return -INFINITY;
+  }
+  return x;
+}
+
 constexpr int kRadixBins = 2048;
 
 // Exact k-th largest logit of a row (1 <= k < V) by radix select over `order_key`: three passes of 11, 11 and 10 bits, each a
 // shared-memory histogram of the keys that match the digits chosen so far, then a suffix scan that finds the digit holding the
-// k-th key. `hist` has kRadixBins words, `sm_u` 34.
-__device__ float radix_kth_largest(const float* __restrict__ lg, int V, int k, uint32_t* hist, uint32_t* sm_u) {
+// k-th key. `hist` has kRadixBins words, `sm_u` 34.  Masked ids count as -inf (`draw_logit`).
+template <bool kMask>
+__device__ float radix_kth_largest(const float* __restrict__ lg, const uint32_t* __restrict__ al, int V, int k, uint32_t* hist,
+                                   uint32_t* sm_u) {
   const int t = threadIdx.x, warp = t >> 5, lane = t & 31;
   uint32_t prefix = 0, mask = 0, rem = (uint32_t)k;  // rem: rank of the wanted key among the keys that match `prefix`
 #pragma unroll 1
@@ -83,7 +98,7 @@ __device__ float radix_kth_largest(const float* __restrict__ lg, int V, int k, u
     for (int i = t; i < kRadixBins; i += kSampThreads) hist[i] = 0u;
     __syncthreads();
     for (int i = t; i < V; i += kSampThreads) {
-      const uint32_t key = order_key(lg[i]);
+      const uint32_t key = order_key(draw_logit<kMask>(lg, al, i));
       if ((key & mask) == prefix) atomicAdd(&hist[(key >> shift) & dmask], 1u);
     }
     __syncthreads();
@@ -116,8 +131,10 @@ __device__ float radix_kth_largest(const float* __restrict__ lg, int V, int k, u
 
 // Temperature draw of one row inside the kept set.  kFilt == false is the plain top-p / categorical path; kFilt == true adds the
 // top-k floor `kth` (the top-p mass sums run over x >= kth only) and keeps x >= floor = max(kth, min-p threshold) in the draw.
-template <bool kFilt>
-__device__ __forceinline__ int draw_token(const float* __restrict__ lg, int V, float amv, float temp, float tp, float kth,
+// kMask: ids masked off in `al` read as -inf, and `amv` is the max over the allowed ids.
+template <bool kFilt, bool kMask>
+__device__ __forceinline__ int draw_token(const float* __restrict__ lg, const uint32_t* __restrict__ al, int V, float amv,
+                                          float temp, float tp, float kth,
                                           float floor, unsigned long long seed, unsigned long long step, uint32_t rng_row,
                                           ArgMax* sm_a, float* sm_f) {
   const float inv_t = 1.0f / temp;
@@ -126,7 +143,7 @@ __device__ __forceinline__ int draw_token(const float* __restrict__ lg, int V, f
     // Z at temperature
     float zs = 0.f;
     for (int i = threadIdx.x; i < V; i += kSampThreads) {
-      const float x = lg[i];
+      const float x = draw_logit<kMask>(lg, al, i);
       if (!kFilt || x >= kth) zs += __expf((x - amv) * inv_t);
     }
     zs = block_sum(zs, sm_f);
@@ -138,7 +155,7 @@ __device__ __forceinline__ int draw_token(const float* __restrict__ lg, int V, f
       const float mid = 0.5f * (lo + hi);
       float ms = 0.f;
       for (int i = threadIdx.x; i < V; i += kSampThreads) {
-        const float x = lg[i];
+        const float x = draw_logit<kMask>(lg, al, i);
         if (x <= mid && (!kFilt || x >= kth)) ms += __expf((x - amv) * inv_t);
       }
       ms = block_sum(ms, sm_f);
@@ -149,7 +166,7 @@ __device__ __forceinline__ int draw_token(const float* __restrict__ lg, int V, f
   // Gumbel-max over the kept set: argmax (logit / T + g), g = -log(-log(u))
   ArgMax gm{-INFINITY, 0x7fffffff};
   for (int i = threadIdx.x; i < V; i += kSampThreads) {
-    const float x = lg[i];
+    const float x = draw_logit<kMask>(lg, al, i);
     if (x > thresh && (!kFilt || x >= floor)) {
       const float u = uniform01(seed, step, rng_row, i);
       const float g = -__logf(-__logf(u));
@@ -160,12 +177,15 @@ __device__ __forceinline__ int draw_token(const float* __restrict__ lg, int V, f
   return gm.i;
 }
 
+// kMask == false is the unmasked sampler; kMask == true reads a token mask `allow` of ceil(V / 32) words per row.
+template <bool kMask>
 __global__ void __launch_bounds__(kSampThreads, 1)
 sample_kernel(const float* __restrict__ logits, int V, const float* __restrict__ temperature, const float* __restrict__ top_p,
               const int* __restrict__ keep_k, const float* __restrict__ min_p,
               unsigned long long seed, unsigned long long step, const unsigned long long* __restrict__ row_rng,
               long long* __restrict__ tokens, float* __restrict__ logprobs, int top_k, long long* __restrict__ top_ids,
-              float* __restrict__ top_lp, const uint4* __restrict__ tag_src, uint4* __restrict__ tag_dst) {
+              float* __restrict__ top_lp, const uint4* __restrict__ tag_src, uint4* __restrict__ tag_dst,
+              const uint32_t* __restrict__ allow) {
   pdl_sync();  // PDL: predecessor's writes visible; let the successor start its prologue
   // Random stream of a row: (seed, step) launch scalars, or — for CUDA-graph replay, where scalars are frozen at capture — a
   // per-row (seed, step) pair in device memory (`row_rng[b]` = request seed, number of tokens that request has sampled so far:
@@ -182,10 +202,26 @@ sample_kernel(const float* __restrict__ logits, int V, const float* __restrict__
   __shared__ float sm_f[kSampThreads / 32];
   const int b = blockIdx.x;
   const float* lg = logits + (size_t)b * V;
-  // pass 1: max / argmax
+  // pass 1: max / argmax of the row (`am`, for the reported log-probs) and of the ids the draw may pick (`dm`)
   ArgMax am{-INFINITY, 0x7fffffff};
-  for (int i = threadIdx.x; i < V; i += kSampThreads) am = better(am, ArgMax{lg[i], i});
-  am = block_argmax(am, sm_a);
+  ArgMax dm{-INFINITY, 0x7fffffff};
+  const uint32_t* al = nullptr;  // mask row, or nullptr when the row is sampled unmasked
+  if constexpr (kMask) {
+    const uint32_t* row = allow + (size_t)b * ((V + 31) >> 5);
+    for (int i = threadIdx.x; i < V; i += kSampThreads) {
+      const float x = lg[i];
+      am = better(am, ArgMax{x, i});
+      if ((row[i >> 5] >> (i & 31)) & 1u) dm = better(dm, ArgMax{x, i});
+    }
+    am = block_argmax(am, sm_a);
+    dm = block_argmax(dm, sm_a);
+    // a row without an allowed id of finite logit is sampled as if it had no mask (the engine refuses what it draws)
+    if (dm.v > -INFINITY) al = row; else dm = am;
+  } else {
+    for (int i = threadIdx.x; i < V; i += kSampThreads) am = better(am, ArgMax{lg[i], i});
+    am = block_argmax(am, sm_a);
+    dm = am;
+  }
   // pass 2: log-sum-exp (temperature is NOT applied to the reported logprobs, reference utils.py:131)
   float se = 0.f;
   for (int i = threadIdx.x; i < V; i += kSampThreads) se += __expf(lg[i] - am.v);
@@ -194,21 +230,22 @@ sample_kernel(const float* __restrict__ logits, int V, const float* __restrict__
 
   const float temp = temperature[b];
   const float tp = top_p[b];
-  int token = am.i;
+  int token = dm.i;
   if (temp > 0.f) {
     // optional per-row filters: keep_k[b] in [1, V) keeps the logits >= the k-th largest (ties kept), min_p[b] in (0, 1] keeps
-    // p >= min_p * p_max at temperature T, i.e. logit >= max + T * ln(min_p); a row with neither runs the plain path
+    // p >= min_p * p_max at temperature T, i.e. logit >= max + T * ln(min_p); a row with neither runs the plain path.  Under a
+    // mask, the k-th largest, the max and the top-p sums are taken over the allowed ids.
     const int kk = keep_k != nullptr ? keep_k[b] : 0;
     const float mp = min_p != nullptr ? min_p[b] : 0.f;
     const bool use_k = kk > 0 && kk < V;
     if (use_k || mp > 0.f) {
       __shared__ uint32_t sm_hist[kRadixBins];
       __shared__ uint32_t sm_u[34];
-      const float kth = use_k ? radix_kth_largest(lg, V, kk, sm_hist, sm_u) : -INFINITY;
-      const float floor = mp > 0.f ? fmaxf(kth, am.v + temp * logf(mp)) : kth;
-      token = draw_token<true>(lg, V, am.v, temp, tp, kth, floor, seed, step, rng_row, sm_a, sm_f);
+      const float kth = use_k ? radix_kth_largest<kMask>(lg, al, V, kk, sm_hist, sm_u) : -INFINITY;
+      const float floor = mp > 0.f ? fmaxf(kth, dm.v + temp * logf(mp)) : kth;
+      token = draw_token<true, kMask>(lg, al, V, dm.v, temp, tp, kth, floor, seed, step, rng_row, sm_a, sm_f);
     } else {
-      token = draw_token<false>(lg, V, am.v, temp, tp, -INFINITY, -INFINITY, seed, step, rng_row, sm_a, sm_f);
+      token = draw_token<false, kMask>(lg, al, V, dm.v, temp, tp, -INFINITY, -INFINITY, seed, step, rng_row, sm_a, sm_f);
     }
   }
   if (threadIdx.x == 0) {
@@ -268,13 +305,19 @@ cudaError_t apply_penalties_launch(float* logits, int B, int V, const int* rep_c
 }
 
 cudaError_t sample_launch(const float* logits, int B, int V, const float* temperature, const float* top_p, const int* keep_k,
-                          const float* min_p, unsigned long long seed, unsigned long long step, const unsigned long long* row_rng,
-                          long long* tokens, float* logprobs, int top_k, long long* top_ids, float* top_lp, const void* tag_src,
-                          void* tag_dst, cudaStream_t s) {
+                          const float* min_p, const uint32_t* allow, unsigned long long seed, unsigned long long step,
+                          const unsigned long long* row_rng, long long* tokens, float* logprobs, int top_k, long long* top_ids,
+                          float* top_lp, const void* tag_src, void* tag_dst, cudaStream_t s) {
   if (B == 0) return cudaSuccess;
   if (top_k > 32) return cudaErrorInvalidValue;
-  (void)launch_pdl(sample_kernel, dim3(B), dim3(kSampThreads), 0, s, logits, V, temperature, top_p, keep_k, min_p, seed, step,
-                   row_rng, tokens, logprobs, top_k, top_ids, top_lp, static_cast<const uint4*>(tag_src), static_cast<uint4*>(tag_dst));
+  if (allow != nullptr)
+    (void)launch_pdl(sample_kernel<true>, dim3(B), dim3(kSampThreads), 0, s, logits, V, temperature, top_p, keep_k, min_p, seed,
+                     step, row_rng, tokens, logprobs, top_k, top_ids, top_lp, static_cast<const uint4*>(tag_src),
+                     static_cast<uint4*>(tag_dst), allow);
+  else
+    (void)launch_pdl(sample_kernel<false>, dim3(B), dim3(kSampThreads), 0, s, logits, V, temperature, top_p, keep_k, min_p, seed,
+                     step, row_rng, tokens, logprobs, top_k, top_ids, top_lp, static_cast<const uint4*>(tag_src),
+                     static_cast<uint4*>(tag_dst), static_cast<const uint32_t*>(nullptr));
   return cudaGetLastError();
 }
 

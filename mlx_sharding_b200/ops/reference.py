@@ -277,19 +277,33 @@ def filter_keep(x: torch.Tensor, t: float, top_p: float, top_k: int, min_p: floa
     return keep
 
 
+def unpack_allow(allow: torch.Tensor, V: int) -> torch.Tensor:
+    """Token mask int32 ``[B, ceil(V/32)]`` (bit ``j & 31`` of word ``j >> 5`` = id ``j`` allowed) -> bool ``[B, V]``."""
+    shifts = torch.arange(32, device=allow.device)
+    bits = (allow.to(torch.int64)[:, :, None] >> shifts) & 1
+    return bits.reshape(allow.shape[0], -1)[:, :V].bool()
+
+
 def sample(logits: torch.Tensor, temperature: torch.Tensor, top_p: torch.Tensor,
            generator: Optional[torch.Generator] = None, top_logprobs: int = 0,
-           top_k: Optional[torch.Tensor] = None, min_p: Optional[torch.Tensor] = None):
+           top_k: Optional[torch.Tensor] = None, min_p: Optional[torch.Tensor] = None,
+           allow: Optional[torch.Tensor] = None):
     """Batched sampler (reference shard/utils.py:126-139 + mlx_lm ``top_p_sampling``).
 
     ``logits`` fp32 ``[B, V]`` *after* bias / repetition penalty.  Per row: ``temp == 0`` -> argmax;
     ``0 < top_p < 1`` -> nucleus; else categorical(softmax(logits / temp)).  ``top_k`` (int ``[B]``, 0 = off) and ``min_p``
-    (float ``[B]``, 0 = off) optionally narrow the draw of a row with ``temp > 0`` (``filter_keep``).
+    (float ``[B]``, 0 = off) optionally narrow the draw of a row with ``temp > 0`` (``filter_keep``).  ``allow`` (int32
+    ``[B, ceil(V/32)]``, see ``unpack_allow``) masks the draw: disallowed ids are ``-inf`` for the argmax and before
+    ``filter_keep``; a row without an allowed id of finite logit is drawn unmasked.
     Returns ``(tokens int64 [B], token_logprob fp32 [B], topk_ids, topk_logprobs)`` where logprobs are
     ``logits - logsumexp(logits)`` (temperature **not** applied — reference utils.py:131)."""
     B, V = logits.shape
     lf = logits.float()
     logprobs = lf - torch.logsumexp(lf, dim=-1, keepdim=True)
+    draw = lf
+    if allow is not None:
+        masked = lf.masked_fill(~unpack_allow(allow, V).to(lf.device), float("-inf"))
+        draw = torch.where((masked > float("-inf")).any(-1, keepdim=True), masked, lf)
     tokens = torch.empty(B, dtype=torch.int64, device=logits.device)
     t_cpu, p_cpu = temperature.tolist(), top_p.tolist()
     k_cpu = top_k.tolist() if top_k is not None else [0] * B
@@ -297,14 +311,14 @@ def sample(logits: torch.Tensor, temperature: torch.Tensor, top_p: torch.Tensor,
     for b in range(B):
         t, p = t_cpu[b], p_cpu[b]
         if t == 0:
-            tokens[b] = torch.argmax(lf[b])
+            tokens[b] = torch.argmax(draw[b])
             continue
         if 0 < k_cpu[b] < V or m_cpu[b] > 0:
-            keep = filter_keep(lf[b], t, p, int(k_cpu[b]), float(m_cpu[b]))
-            probs = torch.softmax((lf[b] / t).masked_fill(~keep, float("-inf")), dim=-1)
+            keep = filter_keep(draw[b], t, p, int(k_cpu[b]), float(m_cpu[b]))
+            probs = torch.softmax((draw[b] / t).masked_fill(~keep, float("-inf")), dim=-1)
             tokens[b] = torch.multinomial(probs, 1, generator=generator).squeeze()
             continue
-        probs = torch.softmax(lf[b] / t, dim=-1)
+        probs = torch.softmax(draw[b] / t, dim=-1)
         if 0 < p < 1.0:
             sp, si = torch.sort(probs, descending=False, stable=True)
             cum = torch.cumsum(sp, dim=0)
@@ -323,7 +337,7 @@ def sample(logits: torch.Tensor, temperature: torch.Tensor, top_p: torch.Tensor,
 
 def sample_block(logits: torch.Tensor, sv, tag_out, toks_out, lp_out, top_ids_out, top_lp_out):
     """Sampling driven by a step block (``parallel/graph_decode.py``): penalties, then per-sequence temperature / top-p (and the
-    optional top-k / min-p filters) with a
+    optional top-k / min-p filters and token mask) with a
     per-request random stream — row ``b`` draws from a generator seeded with its ``(seed, tokens sampled so far)`` pair, so a
     request's tokens do not depend on which batch it decodes in.  Results go into the result-message views."""
     lf = logits.float().clone()
@@ -336,6 +350,8 @@ def sample_block(logits: torch.Tensor, sv, tag_out, toks_out, lp_out, top_ids_ou
         g = torch.Generator(device=lf.device)
         g.manual_seed((rng[b][0] * 1000003 + rng[b][1] * 7919 + 12345) & 0x7FFFFFFFFFFFFFFF)
         filt = dict(top_k=sv.keep_k[b:b + 1], min_p=sv.min_p[b:b + 1]) if sv.has_filter else {}
+        if sv.allow is not None:
+            filt["allow"] = sv.allow[b:b + 1]
         t, lp, ti, tl = sample(lf[b:b + 1], sv.temps[b:b + 1], sv.top_p[b:b + 1], generator=g, top_logprobs=k, **filt)
         toks_out[b], lp_out[b] = t[0], lp[0]
         if k:

@@ -123,6 +123,9 @@ class LockstepGroup:
         params = params or SamplingParams()
         params.validate()
         check_penalty_table(params, max_tokens)
+        if params.response_format is not None:
+            raise ValueError("response_format is not available with --expert-parallel serving (its ranks have no tokenizer to "
+                             "build token masks from)")
         if len(prompt) == 0:
             raise ValueError("empty prompt")
         if len(prompt) + max_tokens > self.engine.max_model_len:

@@ -7,8 +7,8 @@ for a given (group, batch size, block-table width, context bucket, sampling vari
 
 * defines the **step block** (``StepLayout``): ONE int32 vector that carries everything a stage needs for a step — a 16-byte
   step tag, the sampling block (per-sequence temperature / top-p / RNG state and, when any request uses them, repetition-penalty
-  contexts, bias tables — logit_bias folded with presence / frequency penalties — and top-k / min-p filters), the packed
-  ``BatchMeta`` and the token ids.  Stage 0 builds it once per step; every stage
+  contexts, bias tables — logit_bias folded with presence / frequency penalties — top-k / min-p filters and the token masks of
+  structured-output requests), the packed ``BatchMeta`` and the token ids.  Stage 0 builds it once per step; every stage
   copies it host->device with one pinned ``cudaMemcpyAsync``; in a multi-GPU pipeline it travels through the shared-memory
   launch ring (``shm_ring.py``);
 * defines the **result message** (``ResultLayout``): tag + sampled ids + their log-probs (+ top-k) in one buffer the last stage
@@ -53,20 +53,21 @@ class StepLayout:
     ``C`` / ``NB`` > 0: the block carries repetition-penalty contexts ``[B, C]`` and additive bias tables ``[B, NB]`` (logit_bias
     merged with the presence / frequency penalties; only when a request of the batch uses them); ``F`` = 1: it carries the
     top-k / min-p filter section ``keep_k`` int32 ``[B]`` + ``min_p`` f32 ``[B]`` (only when a request of the batch filters its
-    draw); ``k`` = number of top log-probs the sampler returns (0 or 10)."""
+    draw); ``W`` > 0: it carries the token-mask section ``allow`` int32 ``[B, W]``, ``W = ceil(V/32)`` (only when a request of
+    the batch has a ``response_format``); ``k`` = number of top log-probs the sampler returns (0 or 10)."""
 
-    __slots__ = ("T", "B", "mb", "C", "NB", "k", "F", "tag", "temps", "top_p", "rng", "penalty", "rep", "bidx", "bval", "keep_k",
-                 "min_p", "meta", "tokens", "size")
+    __slots__ = ("T", "B", "mb", "C", "NB", "k", "F", "W", "tag", "temps", "top_p", "rng", "penalty", "rep", "bidx", "bval",
+                 "keep_k", "min_p", "allow", "meta", "tokens", "size")
 
-    def __init__(self, T: int, B: int, mb: int, C: int = 0, NB: int = 0, k: int = 0, F: int = 0):
-        self.T, self.B, self.mb, self.C, self.NB, self.k, self.F = T, B, mb, C, NB, k, F
+    def __init__(self, T: int, B: int, mb: int, C: int = 0, NB: int = 0, k: int = 0, F: int = 0, W: int = 0):
+        self.T, self.B, self.mb, self.C, self.NB, self.k, self.F, self.W = T, B, mb, C, NB, k, F, W
         o = 0
         self.tag = o; o += 4                       # [seq_lo, seq_hi, k, flags] — 16 bytes, copied into the result message
         self.temps = o; o += B
         self.top_p = o; o += B
         o = (o + 1) // 2 * 2
         self.rng = o; o += 4 * B                   # int64 [B, 2] = (seed, tokens sampled so far) per sequence
-        self.penalty = self.rep = self.bidx = self.bval = self.keep_k = self.min_p = -1
+        self.penalty = self.rep = self.bidx = self.bval = self.keep_k = self.min_p = self.allow = -1
         if C or NB:
             self.penalty = o; o += B
             self.rep = o; o += B * C
@@ -75,6 +76,9 @@ class StepLayout:
         if F:
             self.keep_k = o; o += B
             self.min_p = o; o += B
+        if W:
+            o = (o + 3) // 4 * 4               # 16-byte aligned
+            self.allow = o; o += B * W
         o = (o + 3) // 4 * 4
         self.meta = o; o += BatchMeta.packed_size(T, B, mb)
         o = (o + 1) // 2 * 2
@@ -82,11 +86,16 @@ class StepLayout:
         self.size = (o + 3) // 4 * 4
 
     @property
-    def key(self) -> Tuple[int, int, int, int, int, int, int]:
-        return (self.T, self.B, self.mb, self.C, self.NB, self.k, self.F)
+    def key(self) -> Tuple[int, int, int, int, int, int, int, int]:
+        return (self.T, self.B, self.mb, self.C, self.NB, self.k, self.W, self.F)
+
+    @property
+    def flags(self) -> int:
+        """Header word 7: bit 0 = filter section present, bits 1-31 = ``W`` of the token-mask section (0 = absent)."""
+        return self.F | (self.W << 1)
 
 
-HEADER_WORDS = 8      # prepended to the block on the wire: T, B, mb, C, NB, k, is_prefill, F (filter section present)
+HEADER_WORDS = 8      # prepended to the block on the wire: T, B, mb, C, NB, k, is_prefill, flags (``StepLayout.flags``)
 
 
 class ResultLayout:
@@ -146,7 +155,7 @@ def decode_bucket(B: int) -> int:
     return (B + 7) // 8 * 8 if B <= 64 else (B + 15) // 16 * 16
 
 
-def _pad_decode(meta: BatchMeta, tokens: torch.Tensor, params, contexts, rng, counts, Bp: int):
+def _pad_decode(meta: BatchMeta, tokens: torch.Tensor, params, contexts, rng, counts, allow, Bp: int):
     """Pad a pure-decode step to ``Bp`` sequences with dummy rows that read / write the reserved null page (page 0, position 0)."""
     B, n = meta.num_seqs, Bp - meta.num_seqs
     z = lambda k: torch.zeros(k, dtype=torch.int32)
@@ -160,17 +169,20 @@ def _pad_decode(meta: BatchMeta, tokens: torch.Tensor, params, contexts, rng, co
     contexts = (list(contexts) + [[]] * n) if contexts is not None else None
     rng = (list(rng) + [(0, 0)] * n) if rng is not None else None
     counts = (list(counts) + [None] * n) if counts is not None else None
-    return meta, tokens, params, contexts, rng, counts
+    if allow is not None:   # dummy rows may draw anything
+        allow = np.concatenate([allow, np.full((n, allow.shape[1]), -1, dtype=np.int32)])
+    return meta, tokens, params, contexts, rng, counts, allow
 
 
 _PAD_PARAMS = None
 
 
 def pack_step(seq: int, meta: BatchMeta, tokens: torch.Tensor, params, contexts, rng, is_prefill: bool,
-              pad_decode: bool = False, counts=None) -> Tuple[np.ndarray, StepLayout]:
+              pad_decode: bool = False, counts=None, allow: Optional[np.ndarray] = None) -> Tuple[np.ndarray, StepLayout]:
     """Host side (stage 0): one int32 vector ``[header | step block]`` for this step.  ``rng[b]`` = (seed, sampled so far);
     ``counts[b]`` = ``OutputCounts`` of a request with a presence / frequency penalty (else ``None``), folded with
-    its ``logit_bias`` into one bias entry per token id.
+    its ``logit_bias`` into one bias entry per token id; ``allow`` = token masks int32 ``[B, ceil(V/32)]`` of a batch with a
+    structured-output request (rows of the other requests all ones), else ``None``.
 
     ``pad_decode``: a pure decode step is padded to the next batch-size bucket (``decode_bucket``) with dummy rows on the null
     page, so that continuous batching — sequences joining and leaving every few steps — keeps replaying a handful of captured
@@ -183,14 +195,15 @@ def pack_step(seq: int, meta: BatchMeta, tokens: torch.Tensor, params, contexts,
                 from ..engine.sampler import SamplingParams
 
                 _PAD_PARAMS = SamplingParams()
-            meta, tokens, params, contexts, rng, counts = _pad_decode(meta, tokens, params, contexts, rng, counts, Bp)
+            meta, tokens, params, contexts, rng, counts, allow = _pad_decode(meta, tokens, params, contexts, rng, counts, allow, Bp)
     T, B = meta.num_tokens, meta.num_seqs
     mb = meta.block_tables.shape[1]
     C, NB, k = sampling_variant(params, counts)
     F = int(any(p.uses_filter for p in params))
-    lay = StepLayout(T, B, mb, C, NB, k, F)
+    W = 0 if allow is None else int(allow.shape[1])
+    lay = StepLayout(T, B, mb, C, NB, k, F, W)
     buf = np.zeros(HEADER_WORDS + lay.size, dtype=np.int32)
-    buf[:HEADER_WORDS] = (T, B, mb, C, NB, k, int(is_prefill), F)
+    buf[:HEADER_WORDS] = (T, B, mb, C, NB, k, int(is_prefill), lay.flags)
     blk = buf[HEADER_WORDS:]
     blk[lay.tag] = seq & 0x7FFFFFFF
     blk[lay.tag + 1] = (seq >> 31) & 0x7FFFFFFF
@@ -220,14 +233,16 @@ def pack_step(seq: int, meta: BatchMeta, tokens: torch.Tensor, params, contexts,
     if F:
         blk[lay.keep_k:lay.keep_k + B] = [max(p.top_k, 0) if p.uses_filter else 0 for p in params]
         f32[lay.min_p:lay.min_p + B] = [p.min_p if p.uses_filter else 0.0 for p in params]
+    if W:
+        blk[lay.allow:lay.allow + B * W].reshape(B, W)[:] = allow
     blk[lay.meta:lay.meta + BatchMeta.packed_size(T, B, mb)] = meta.pack().numpy()
     blk[lay.tokens:lay.tokens + 2 * T].view(np.int64)[:] = tokens.numpy()
     return buf, lay
 
 
 def unpack_header(buf: np.ndarray) -> Tuple[StepLayout, bool]:
-    T, B, mb, C, NB, k, pre, F = (int(v) for v in buf[:HEADER_WORDS])
-    return StepLayout(T, B, mb, C, NB, k, F), bool(pre)
+    T, B, mb, C, NB, k, pre, flags = (int(v) for v in buf[:HEADER_WORDS])
+    return StepLayout(T, B, mb, C, NB, k, flags & 1, flags >> 1), bool(pre)
 
 
 class StepViews:
@@ -250,6 +265,7 @@ class StepViews:
         self.has_filter = bool(lay.F)
         self.keep_k = flat[lay.keep_k:lay.keep_k + B] if lay.F else None
         self.min_p = f32[lay.min_p:lay.min_p + B] if lay.F else None
+        self.allow = flat[lay.allow:lay.allow + B * lay.W].view(B, lay.W) if lay.W else None
         o = lay.meta + 6
         take = lambda n: (flat[o:o + n], o + n)
         pos, o = take(T)

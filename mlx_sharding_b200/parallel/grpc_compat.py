@@ -290,7 +290,7 @@ class GrpcRelayPipeline:
                 x = s.send_tensor(x, dev)
             x = x[0]
         logits = x[-1:].float()
-        so = self.sampler(logits, inp.params, inp.contexts, inp.counts)
+        so = self.sampler(logits, inp.params, inp.contexts, inp.counts, allow=inp.allow)
         return StepOutput(so.tokens.tolist(), so.logprobs.tolist(),
                           None if so.top_ids is None else so.top_ids.tolist(),
                           None if so.top_logprobs is None else so.top_logprobs.tolist())

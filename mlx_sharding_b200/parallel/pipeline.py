@@ -217,7 +217,7 @@ class LocalPipeline:
     def submit(self, inp: StepInput) -> StepOutput:
         self._seq += 1
         wire, lay = pack_step(self._seq, inp.meta, inp.tokens, inp.params, inp.contexts, inp.rng, inp.is_prefill,
-                              pad_decode=self.gcache is not None and self.gcache.enabled, counts=inp.counts)
+                              pad_decode=self.gcache is not None and self.gcache.enabled, counts=inp.counts, allow=inp.allow)
         x = None
         for r in self.runners:
             x = r.run(wire, inp.group, x_local=None if x is None else x.to(r.dev))
@@ -413,13 +413,14 @@ class DistControl:
         pass
 
 
-def control_slot_bytes(max_tokens: int, max_seqs: int) -> int:
+def control_slot_bytes(max_tokens: int, max_seqs: int, vocab_size: int = 0) -> int:
     """Bytes of a control-ring slot: it holds the largest step block — a prefill chunk of ``max_tokens`` tokens (+ block tables
     of ``max_seqs`` sequences) — plus the sampling tables of ``max_seqs`` rows at their largest: a 32-token repetition context,
-    a bias table of ``MAX_PENALTY_TABLE`` entries (penalised requests are refused beyond it) and the top-k / min-p section.
-    The ring file is sparse, so slot bytes a step does not write take no memory."""
+    a bias table of ``MAX_PENALTY_TABLE`` entries (penalised requests are refused beyond it), the top-k / min-p section and a
+    token mask of ``ceil(vocab_size / 32)`` words (structured output).  The ring file is sparse, so slot bytes a step does not
+    write take no memory."""
     base = max(256 << 10, 16 * max_tokens + 1024 * max_seqs + 4096)
-    sampling = 4 * max_seqs * (1 + 32 + 2 * MAX_PENALTY_TABLE + 2)
+    sampling = 4 * max_seqs * (1 + 32 + 2 * MAX_PENALTY_TABLE + 2) + 4 * max_seqs * ((vocab_size + 31) // 32) + 16
     return (base + sampling + 4095) // 4096 * 4096
 
 
@@ -448,7 +449,7 @@ def build_chain(stage: StageExecutor, num_groups: Optional[int] = None, max_toke
         box = [None]
         ctl = None
         if rank == 0:
-            ctl = ShmControl.create(world, slots=128, slot_bytes=control_slot_bytes(max_tokens, max_seqs))
+            ctl = ShmControl.create(world, slots=128, slot_bytes=control_slot_bytes(max_tokens, max_seqs, stage.model.cfg.vocab_size))
             box[0] = ctl.path
         dist.broadcast_object_list(box, 0, group=ctrl_group)
         if rank != 0:
@@ -504,7 +505,7 @@ class ChainPipeline:
         self._seq += 1
         seq = self._seq
         wire, lay = pack_step(seq, inp.meta, inp.tokens, inp.params, inp.contexts, inp.rng, inp.is_prefill,
-                              pad_decode=self.gcache.enabled, counts=inp.counts)
+                              pad_decode=self.gcache.enabled, counts=inp.counts, allow=inp.allow)
         self.ctl.publish(KIND_STEP, inp.group, wire)
         try:
             self.runner.run(wire, inp.group)

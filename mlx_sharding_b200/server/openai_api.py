@@ -34,6 +34,7 @@ from typing import Dict, List, Optional
 import torch
 
 from ..engine.core import LLMEngine, stopping_criteria
+from ..engine.grammar import canonical_format
 from ..engine.sampler import SamplingParams
 
 log = logging.getLogger("mlx_sharding_b200.api")
@@ -116,6 +117,11 @@ def parse_request_params(body: dict) -> dict:
     for name in ("presence_penalty", "frequency_penalty"):
         if not num(p[name]) or not -2 <= p[name] <= 2:
             raise RequestError(f"{name} must be a float between -2 and 2")
+    # structured output: {"type": "text" | "json_object" | "json_schema", "json_schema": {...}} (engine/grammar.py)
+    try:
+        p["response_format"] = canonical_format(body.get("response_format"))
+    except ValueError as e:
+        raise RequestError(str(e)) from None
     return p
 
 
@@ -249,7 +255,13 @@ class ModelProvider:
             tokenizer = load_tokenizer(get_model_path(path), tok_cfg)
             if getattr(a, "use_default_chat_template", False) and tokenizer.chat_template is None:
                 tokenizer.chat_template = getattr(tokenizer, "default_chat_template", None)
-            engine = self._build_engine(model).start()
+            engine = self._build_engine(model)
+            if isinstance(engine, LLMEngine):
+                # structured output: token masks from the tokenizer's vocabulary at the model's vocab_size (None without xgrammar)
+                from ..engine.grammar import GrammarBackend
+
+                engine.grammar = GrammarBackend.create(tokenizer, model.cfg.vocab_size)
+            engine.start()
             self.model_key, self.model, self.tokenizer, self.engine = model_path, model, tokenizer, engine
             return model, tokenizer, engine
 
@@ -390,7 +402,8 @@ class APIHandler(BaseHTTPRequestHandler):
                                     logit_bias=prm["logit_bias"], logprobs=max(prm["logprobs"], 0), seed=prm["seed"],
                                     top_k=prm["top_k"], min_p=float(prm["min_p"]),
                                     presence_penalty=float(prm["presence_penalty"]),
-                                    frequency_penalty=float(prm["frequency_penalty"]))
+                                    frequency_penalty=float(prm["frequency_penalty"]),
+                                    response_format=prm["response_format"])
             req = self.engine.submit(prompt, params, max_tokens=prm["max_tokens"],
                                      eos_token_id=self.tokenizer.eos_token_id, stop_id_sequences=stop_ids)
         except (RequestError, ValueError, AssertionError, KeyError) as e:

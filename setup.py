@@ -11,6 +11,8 @@ setup(
     py_modules=["generate", "sharding_weight"],
     python_requires=">=3.10",
     install_requires=["torch", "numpy", "safetensors", "transformers", "grpcio", "protobuf"],
+    # optional: ``response_format`` (structured output) on the OpenAI server; --model <hub repo id>
+    extras_require={"structured": ["xgrammar>=0.2"], "hub": ["huggingface_hub"]},
     entry_points={
         "console_scripts": [
             "mlx-sharding-server=shard.main:main",
