@@ -197,13 +197,9 @@ flash_prefill_kernel(const __nv_bfloat16* __restrict__ q, long long q_ld_t, long
 template <int DK, int DV>
 cudaError_t launch_prefill(const FlashPrefillArgs& a, cudaStream_t s) {
   constexpr int smem = 2 * kBN * ((DK + 8) + (DV + 8)) * 2;
-  auto kern = flash_prefill_kernel<DK, DV>;
-  static bool configured = false;
-  if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) return e;
-    configured = true;
-  }
+  constexpr auto kern = flash_prefill_kernel<DK, DV>;
+  cudaError_t e = set_max_dynamic_smem_once<kern>(smem);
+  if (e != cudaSuccess) return e;
   dim3 grid(a.max_tiles, a.q_heads);
   (void)launch_pdl(kern, dim3(grid), dim3(kThreads), smem, s, static_cast<const __nv_bfloat16*>(a.q), a.q_ld_t, a.q_ld_h,
                                     static_cast<const __nv_bfloat16*>(a.kpool), static_cast<const __nv_bfloat16*>(a.vpool),

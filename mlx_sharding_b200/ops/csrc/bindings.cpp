@@ -66,56 +66,28 @@ Scratch& scratch() {
   return s;
 }
 
-int sm_count() {
-  static int n = 0;
-  if (n == 0) n = at::cuda::getCurrentDeviceProperties()->multiProcessorCount;
-  return n;
-}
-
-// Token tile of the grouped (MoE) GEMMs: ~2x the average rows per expert but never below 64, so an expert's rows rarely need a
-// second tile; gemm_clamp_bn caps it at what the register accumulators allow.
-int grouped_bn(int64_t max_rows, int64_t R, int64_t E) {
-  return b200::gemm_pick_bn((int)std::min<int64_t>(max_rows, std::max<int64_t>(64, 2 * ((R + E - 1) / E))));
-}
-
-int auto_splits(int rows, int n, int k, bool grouped) {
-  if (grouped || rows > 256) return 1;
-  const int tiles = (n + 127) / 128;
-  const int kb = (k + 63) / 64;
-  int s = 1;
-  // fill ~one wave of SMs while keeping >= 8 k-blocks per split
-  while (tiles * (s * 2) <= sm_count() && kb / (s * 2) >= 8 && s < 4) s *= 2;
-  return s;
-}
-
 // ---- GEMM -------------------------------------------------------------------------------------------------------
-Tensor linear(const Tensor& x, const Tensor& w, const c10::optional<Tensor>& w2, const c10::optional<Tensor>& residual,
-              const c10::optional<Tensor>& bias, int64_t act, double softcap, bool out_fp32, const c10::optional<Tensor>& out_,
-              int64_t splits, int64_t signal_flag_ptr, int64_t signal_value) {
-  check_bf16(x, "x"); check_bf16(w, "w"); check_rows(x, "x"); check_rows(w, "w");
-  const c10::cuda::CUDAGuard guard(x.device());
-  const int64_t T = x.size(0), K = x.size(1), N = w.size(0);
-  TORCH_CHECK(w.size(1) == K, "x/w inner dims differ");
+// Shared by linear / linear_q: the output tensor, epilogue operands, split-K scratch and the fused-signal counter of a dense
+// launch whose weight fields (w, w2, n, quantisation) are already in `a`.
+Tensor dense_linear(b200::GemmArgs& a, b200::GemmKind kind, const Tensor& x, const c10::optional<Tensor>& residual,
+                    const c10::optional<Tensor>& bias, int64_t act, double softcap, bool out_fp32, const c10::optional<Tensor>& out_,
+                    int64_t splits, int64_t signal_flag_ptr, int64_t signal_value) {
+  const int64_t T = x.size(0), K = x.size(1), N = a.n;
   Tensor out = out_.has_value() ? *out_ : torch::empty({T, N}, x.options().dtype(out_fp32 ? torch::kFloat32 : torch::kBFloat16));
   TORCH_CHECK(out.dim() == 2 && out.stride(1) == 1 && out.size(0) >= T && out.size(1) == N, "bad out tensor");
   if (T == 0) return out;
-  b200::GemmArgs a;
   a.x = x.data_ptr(); a.x_rows = T; a.ld_x = x.stride(0);
-  a.w = w.data_ptr(); a.ld_w = w.stride(0);
-  if (w2.has_value()) { check_bf16(*w2, "w2"); TORCH_CHECK(w2->sizes() == w.sizes() && w2->stride(0) == w.stride(0)); a.w2 = w2->data_ptr(); }
-  a.m = (int)T; a.n = (int)N; a.k = (int)K; a.max_rows = (int)T;
+  a.m = (int)T; a.k = (int)K; a.max_rows = (int)T;
   a.out = out.data_ptr(); a.ld_out = out.stride(0); a.out_fp32 = out.scalar_type() == torch::kFloat32;
   if (residual.has_value()) { check_bf16(*residual, "residual"); check_rows(*residual, "residual"); a.residual = residual->data_ptr(); a.ld_res = residual->stride(0); }
   if (bias.has_value()) { check_bf16(*bias, "bias"); a.bias = bias->data_ptr(); }
   a.act = (int)act; a.softcap = (float)softcap;
-  int sp = splits > 0 ? (int)splits : auto_splits((int)T, (int)N, (int)K, false);
-  a.splits = sp;
+  a.splits = (int)splits;
+  const b200::GemmPlan plan = b200::gemm_plan(a, kind, b200::sm_count());
   auto& sc = scratch();
   Tensor ctr = sc.get_counters(x.device());
-  if (sp > 1) {
-    const int bn = b200::gemm_pick_bn((int)T);
-    Tensor ws = sc.get_ws((int64_t)b200::gemm_workspace_floats(a, bn, sp), x.device());
-    a.workspace = ws.data_ptr<float>();
+  if (plan.route == b200::kRouteWorkspaceSplitK) {
+    a.workspace = sc.get_ws((int64_t)plan.workspace_floats, x.device()).data_ptr<float>();
     a.tile_counters = reinterpret_cast<unsigned int*>(ctr.data_ptr<int>());
   }
   if (signal_flag_ptr != 0) {
@@ -123,8 +95,20 @@ Tensor linear(const Tensor& x, const Tensor& w, const c10::optional<Tensor>& w2,
     a.signal_value = (uint32_t)signal_value;
     a.done_counter = reinterpret_cast<unsigned int*>(ctr.data_ptr<int>()) + 65535;
   }
-  LAUNCH_OK(b200::gemm_launch(a, cur_stream()));
+  LAUNCH_OK(kind == b200::kGemmQuant ? b200::gemm_q_launch(a, plan, cur_stream()) : b200::gemm_launch(a, plan, cur_stream()));
   return out;
+}
+
+Tensor linear(const Tensor& x, const Tensor& w, const c10::optional<Tensor>& w2, const c10::optional<Tensor>& residual,
+              const c10::optional<Tensor>& bias, int64_t act, double softcap, bool out_fp32, const c10::optional<Tensor>& out_,
+              int64_t splits, int64_t signal_flag_ptr, int64_t signal_value) {
+  check_bf16(x, "x"); check_bf16(w, "w"); check_rows(x, "x"); check_rows(w, "w");
+  const c10::cuda::CUDAGuard guard(x.device());
+  TORCH_CHECK(w.size(1) == x.size(1), "x/w inner dims differ");
+  b200::GemmArgs a;
+  a.w = w.data_ptr(); a.ld_w = w.stride(0); a.n = (int)w.size(0);
+  if (w2.has_value()) { check_bf16(*w2, "w2"); TORCH_CHECK(w2->sizes() == w.sizes() && w2->stride(0) == w.stride(0)); a.w2 = w2->data_ptr(); }
+  return dense_linear(a, b200::kGemmBf16, x, residual, bias, act, softcap, out_fp32, out_, splits, signal_flag_ptr, signal_value);
 }
 
 Tensor grouped_linear(const Tensor& x, const Tensor& w, const c10::optional<Tensor>& w2, const Tensor& expert_offsets,
@@ -166,12 +150,10 @@ Tensor grouped_linear(const Tensor& x, const Tensor& w, const c10::optional<Tens
     a.num_signal_peers = (int)signal_peers->numel();
     a.done_counter = reinterpret_cast<unsigned int*>(done_counter->data_ptr<int>());
   }
-  // token tile sized for ~2x the average rows per expert (not the worst case): less padding in the MMA N dimension and
-  // smaller token-tile loads; experts with more rows simply take further tiles of the persistent tile list
   // expected_rows (>0): the caller's estimate of the rows actually present when x is an over-sized buffer (EP receive side)
-  a.bn = grouped_bn(a.max_rows, expected_rows > 0 ? expected_rows : R, E);
-  a.out = out.data_ptr(); a.ld_out = N; a.out_fp32 = out_fp32; a.act = (int)act; a.splits = 1;
-  LAUNCH_OK(b200::gemm_launch(a, cur_stream()));
+  a.expected_rows = expected_rows > 0 ? expected_rows : R;
+  a.out = out.data_ptr(); a.ld_out = N; a.out_fp32 = out_fp32; a.act = (int)act;
+  LAUNCH_OK(b200::gemm_launch(a, b200::gemm_plan(a, b200::kGemmBf16, b200::sm_count()), cur_stream()));
   return out;
 }
 
@@ -189,43 +171,16 @@ Tensor linear_q(const Tensor& x, const Tensor& wq, const Tensor& scales_t, const
                 const c10::optional<Tensor>& out_, int64_t splits, int64_t signal_flag_ptr, int64_t signal_value) {
   check_bf16(x, "x"); check_rows(x, "x");
   const c10::cuda::CUDAGuard guard(x.device());
-  const int64_t T = x.size(0), K = x.size(1);
+  const int64_t K = x.size(1);
   check_q(wq, scales_t, biases_t, N, K, bits, group);
-  Tensor out = out_.has_value() ? *out_ : torch::empty({T, N}, x.options().dtype(out_fp32 ? torch::kFloat32 : torch::kBFloat16));
-  TORCH_CHECK(out.dim() == 2 && out.stride(1) == 1 && out.size(0) >= T && out.size(1) == N, "bad out tensor");
-  if (T == 0) return out;
   b200::GemmArgs a;
-  a.x = x.data_ptr(); a.x_rows = T; a.ld_x = x.stride(0);
-  a.w = wq.data_ptr(); a.q_scales_t = scales_t.data_ptr(); a.q_biases_t = biases_t.data_ptr();
+  a.w = wq.data_ptr(); a.q_scales_t = scales_t.data_ptr(); a.q_biases_t = biases_t.data_ptr(); a.n = (int)N;
   a.q_bits = (int)bits; a.q_group = (int)group;
   if (wq2.has_value()) {
     check_q(*wq2, *scales2_t, *biases2_t, N, K, bits, group);
     a.w2 = wq2->data_ptr(); a.q_scales2_t = scales2_t->data_ptr(); a.q_biases2_t = biases2_t->data_ptr();
   }
-  a.m = (int)T; a.n = (int)N; a.k = (int)K; a.max_rows = (int)T;
-  a.out = out.data_ptr(); a.ld_out = out.stride(0); a.out_fp32 = out.scalar_type() == torch::kFloat32;
-  if (residual.has_value()) { check_bf16(*residual, "residual"); check_rows(*residual, "residual"); a.residual = residual->data_ptr(); a.ld_res = residual->stride(0); }
-  if (bias.has_value()) { check_bf16(*bias, "bias"); a.bias = bias->data_ptr(); }
-  a.act = (int)act; a.softcap = (float)softcap;
-  // quantised weights: 3.5x fewer bytes per tile, so batches of >= 64 tokens use the persistent kernel un-split; tiny decode
-  // batches are latency-bound per tile like the bf16 path and take the same split-K heuristic
-  int sp = splits > 0 ? (int)splits : (T <= 32 ? auto_splits((int)T, (int)N, (int)K, false) : 1);
-  a.splits = sp;
-  auto& sc = scratch();
-  Tensor ctr = sc.get_counters(x.device());
-  if (sp > 1) {
-    const int bn = b200::gemm_pick_bn((int)T);
-    Tensor ws = sc.get_ws((int64_t)b200::gemm_workspace_floats(a, bn, sp), x.device());
-    a.workspace = ws.data_ptr<float>();
-    a.tile_counters = reinterpret_cast<unsigned int*>(ctr.data_ptr<int>());
-  }
-  if (signal_flag_ptr != 0) {
-    a.signal_flag = reinterpret_cast<uint32_t*>(signal_flag_ptr);
-    a.signal_value = (uint32_t)signal_value;
-    a.done_counter = reinterpret_cast<unsigned int*>(ctr.data_ptr<int>()) + 65535;
-  }
-  LAUNCH_OK(b200::gemm_q_launch(a, cur_stream()));
-  return out;
+  return dense_linear(a, b200::kGemmQuant, x, residual, bias, act, softcap, out_fp32, out_, splits, signal_flag_ptr, signal_value);
 }
 
 Tensor grouped_linear_q(const Tensor& x, const Tensor& wq, const Tensor& scales_t, const Tensor& biases_t, const c10::optional<Tensor>& wq2,
@@ -248,14 +203,33 @@ Tensor grouped_linear_q(const Tensor& x, const Tensor& wq, const Tensor& scales_
   }
   a.m = (int)R; a.n = (int)N; a.k = (int)K; a.max_rows = (int)std::min<int64_t>(max_rows, R);
   a.num_experts = (int)E; a.expert_offsets = expert_offsets.data_ptr<int>();
-  // token tile sized for ~2x the average rows per expert (not the worst case): less padding in the MMA N dimension and
-  // smaller token-tile loads; experts with more rows simply take further tiles of the persistent tile list
-  a.bn = grouped_bn(a.max_rows, R, E);
-  a.out = out.data_ptr(); a.ld_out = N; a.out_fp32 = out_fp32; a.act = (int)act; a.splits = 1;
-  LAUNCH_OK(b200::gemm_q_launch(a, cur_stream()));
+  a.expected_rows = R;
+  a.out = out.data_ptr(); a.ld_out = N; a.out_fp32 = out_fp32; a.act = (int)act;
+  LAUNCH_OK(b200::gemm_q_launch(a, b200::gemm_plan(a, b200::kGemmQuant, b200::sm_count()), cur_stream()));
   return out;
 }
 bool gemm_q_supported(int64_t bits, int64_t group, int64_t k) { return b200::gemm_q_supported((int)bits, (int)group, (int)k); }
+
+// The launch plan the bindings above would use, from the GemmArgs fields the planner reads (kind: "bf16", "q" or "fp8").
+py::dict gemm_plan(const std::string& kind, int64_t max_rows, int64_t n, int64_t k, bool pair, int64_t splits, int64_t num_experts,
+                   int64_t expected_rows, int64_t sm_count) {
+  TORCH_CHECK(kind == "bf16" || kind == "q" || kind == "fp8", "kind must be bf16, q or fp8");
+  b200::GemmArgs a;
+  a.max_rows = (int)max_rows; a.n = (int)n; a.k = (int)k; a.splits = (int)splits;
+  a.w2 = pair ? &a : nullptr;   // only its presence is read
+  a.num_experts = (int)num_experts; a.expected_rows = expected_rows;
+  const b200::GemmPlan pl =
+      b200::gemm_plan(a, kind == "bf16" ? b200::kGemmBf16 : kind == "q" ? b200::kGemmQuant : b200::kGemmFp8, (int)sm_count);
+  const char* routes[] = {"persistent", "cluster", "workspace"};
+  py::dict d;
+  d["route"] = routes[pl.route];
+  d["bn"] = pl.bn;
+  d["splits"] = pl.splits;
+  d["grid"] = py::make_tuple(pl.grid.x, pl.grid.y, pl.grid.z);
+  d["cluster"] = pl.cluster_z;
+  d["workspace_floats"] = pl.workspace_floats;
+  return d;
+}
 
 // ---- elementwise ------------------------------------------------------------------------------------------------
 Tensor rmsnorm(const Tensor& x, const Tensor& w, double eps, bool gemma, const c10::optional<Tensor>& residual,
@@ -367,11 +341,11 @@ Tensor linear_fp8(const Tensor& xq, const Tensor& xsf, const Tensor& wq, const T
   if (grouped) {
     TORCH_CHECK(expert_offsets->scalar_type() == torch::kInt32 && (expert_stride > 0 ? expert_offsets->numel() >= E : expert_offsets->numel() == E + 1));
     a.num_experts = (int)E; a.expert_offsets = expert_offsets->data_ptr<int>(); a.expert_stride = (int)expert_stride;
-    a.bn = grouped_bn(a.max_rows, expected_rows > 0 ? expected_rows : R, E);
+    a.expected_rows = expected_rows > 0 ? expected_rows : R;
   }
   if (residual.has_value()) { check_bf16(*residual, "residual"); check_rows(*residual, "residual"); a.residual = residual->data_ptr(); a.ld_res = residual->stride(0); }
   a.out = out.data_ptr(); a.ld_out = N; a.out_fp32 = out_fp32; a.act = (int)act;
-  LAUNCH_OK(b200::gemm_fp8_launch(a, cur_stream()));
+  LAUNCH_OK(b200::gemm_fp8_launch(a, b200::gemm_plan(a, b200::kGemmFp8, b200::sm_count()), cur_stream()));
   return out;
 }
 
@@ -396,7 +370,7 @@ Tensor paged_attention(const Tensor& q, const Tensor& kpool, const Tensor& vpool
   // split the KV range until ~2 waves of CTAs exist, keeping >= 256 positions per split
   int nsplit = 1;
   const int ctas = T * Hk;
-  while (ctas * nsplit < 2 * sm_count() && max_ctx / (nsplit * 2) >= 256 && nsplit < 32) nsplit *= 2;
+  while (ctas * nsplit < 2 * b200::sm_count() && max_ctx / (nsplit * 2) >= 256 && nsplit < 32) nsplit *= 2;
   a.nsplit = nsplit;
   a.out = out.data_ptr(); a.o_ld_t = (long long)Hq * dv;
   a.part_acc = nullptr; a.part_ml = nullptr;
@@ -469,7 +443,7 @@ Tensor mla_decode(const Tensor& q, const Tensor& pool, const Tensor& block_table
     // 19.5 us in two splits, 64 x 1024 best at 2, 64 x 4096 at 2-4, 8 x 16 k at 16 — i.e. ~8+ tiles per split.  `max_ctx` is
     // the *bound* the caller's block tables allow (serving pads them to 8 pages), so short contexts must not split on it.
     nsplit = 1;
-    while (B * nsplit < sm_count() && tiles / (nsplit * 2) >= 8 && nsplit < 64) nsplit *= 2;
+    while (B * nsplit < b200::sm_count() && tiles / (nsplit * 2) >= 8 && nsplit < 64) nsplit *= 2;
   }
   if (nsplit > tiles) nsplit = tiles > 0 ? tiles : 1;
   float* ws = nullptr;
@@ -820,6 +794,8 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("linear_q", &linear_q);
   m.def("grouped_linear_q", &grouped_linear_q);
   m.def("gemm_q_supported", &gemm_q_supported);
+  m.def("gemm_plan", &gemm_plan, py::arg("kind"), py::arg("max_rows"), py::arg("n"), py::arg("k"), py::arg("pair") = false,
+        py::arg("splits") = 0, py::arg("num_experts") = 0, py::arg("expected_rows") = 0, py::arg("sm_count") = 132);
   m.def("rmsnorm", &rmsnorm, py::arg("x"), py::arg("w"), py::arg("eps"), py::arg("gemma") = false, py::arg("residual") = py::none(),
         py::arg("out") = py::none(), py::arg("signal_flag_ptr") = 0, py::arg("signal_value") = 0);
   m.def("rope_", &rope_);

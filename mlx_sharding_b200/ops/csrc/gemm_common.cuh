@@ -18,6 +18,8 @@ constexpr int kProducerWarp = 4;
 constexpr int kATileBytes = kTileM * kBlockK * 2;  // 16 KB
 // Register accumulators bound the token tile: 128 x BN fp32 over 128 threads is BN registers per weight matrix.
 constexpr int kMaxBN = 128, kMaxBNDual = 64;
+// MXFP8 (gemm_fp8.cu): the per-block product needs a second register tile next to the accumulator
+constexpr int kFp8MaxBN = 64, kFp8MaxBNDual = 32;
 
 __host__ __device__ constexpr int acc_bytes(int BN, bool dual) { return BN * (dual ? 2 : 1) * kTileM * 4; }
 __host__ __device__ constexpr int stage_bytes(int BN, bool dual) {
@@ -239,6 +241,39 @@ __device__ __forceinline__ void run_epilogue(const GemmParams& p, const float* a
         }
       }
     }
+}
+
+// ---- host: token tile x pair x output type -> kernel instance
+template <int BN_, bool DUAL_, typename OutT_>
+struct TileCfg {
+  static constexpr int BN = BN_;
+  static constexpr bool DUAL = DUAL_;
+  using OutT = OutT_;
+};
+
+template <bool DUAL, typename OutT, int MaxBN, typename F>
+cudaError_t dispatch_bn(int bn, F& launch) {
+  switch (bn) {
+    case 16: return launch(TileCfg<16, DUAL, OutT>{});
+    case 32: return launch(TileCfg<32, DUAL, OutT>{});
+    case 64:
+      if constexpr (MaxBN >= 64) return launch(TileCfg<64, DUAL, OutT>{});
+      break;
+    case 128:
+      if constexpr (MaxBN >= 128) return launch(TileCfg<128, DUAL, OutT>{});
+      break;
+  }
+  return cudaErrorInvalidValue;
+}
+
+// Calls launch(TileCfg<BN, DUAL, OutT>{}) for the family's kernel instance: fp32 output (single matrix only), gate/up pair
+// into bf16, or a single matrix into bf16.  A family compiles token tiles up to MaxBN (MaxBNDual for a pair); any other bn
+// has no instance and returns cudaErrorInvalidValue.
+template <int MaxBN, int MaxBNDual, typename F>
+cudaError_t dispatch_tile(int bn, bool dual, bool out_fp32, F launch) {
+  if (out_fp32) return dispatch_bn<false, float, MaxBN>(bn, launch);
+  if (dual) return dispatch_bn<true, __nv_bfloat16, MaxBNDual>(bn, launch);
+  return dispatch_bn<false, __nv_bfloat16, MaxBN>(bn, launch);
 }
 
 }  // namespace gemm

@@ -13,8 +13,6 @@
 //
 // Everything else — persistent tile walk, grouped (MoE) mode incl. the fixed-stride scatter layout, DUAL gate/up with act(g)*u
 // epilogue, residual / fp32 outputs — is shared by construction with gemm_persistent.cu.
-#include <algorithm>
-
 #include "gemm_common.cuh"
 #include "gemm_tmap.h"
 #include "launch.h"
@@ -27,8 +25,6 @@ namespace {
 
 constexpr int kFp8Threads = kNumThreads;
 constexpr int kFp8BlockK = 128;             // e4m3 elements per k-block = one 128 B swizzle row
-// the per-block product needs a second register tile next to the accumulator
-constexpr int kFp8MaxBN = 64, kFp8MaxBNDual = 32;
 
 __host__ __device__ constexpr int p_stg_rows(int BN) { return BN < 64 ? BN : 64; }
 __host__ __device__ constexpr int p_staging_bytes(int BN, int out_bytes) { return p_stg_rows(BN) * kTileM * out_bytes; }
@@ -315,93 +311,41 @@ gemm_fp8_persistent_kernel(const __grid_constant__ CUtensorMap tmap_w, const __g
 // ================================================================================================ host side
 namespace {
 
-int sm_count_cached_fp8() {
-  static int n = 0;
-  if (n == 0) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 132;
-  }
-  return n;
-}
-
 template <int BN, bool DUAL, typename OutT>
-cudaError_t f_launch_one(const CUtensorMap& tw, const CUtensorMap& tw2, const CUtensorMap& tx, const GemmParams& p, int tiles_n,
-                         int tiles_m, int num_tiles, cudaStream_t stream) {
+cudaError_t f_launch_one(const GemmMaps& t, const GemmParams& p, const GemmPlan& plan, cudaStream_t stream) {
   constexpr int STAGES = p_num_stages(BN, DUAL, sizeof(OutT));
   constexpr int smem = STAGES * stage_bytes(BN, DUAL) + acc_bytes(BN, DUAL) + p_staging_bytes(BN, sizeof(OutT)) + 2 * STAGES * 8 + 1024;
   static_assert(smem <= 227 * 1024, "shared memory budget exceeded");
-  auto kern = gemm_fp8_persistent_kernel<BN, DUAL, OutT>;
-  static bool configured = false;
-  if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) return e;
-    configured = true;
-  }
-  const int grid = std::min(num_tiles, sm_count_cached_fp8());
-  (void)launch_pdl(kern, dim3(grid), dim3(kFp8Threads), smem, stream, tw, tw2, tx, p, tiles_n, tiles_m, num_tiles);
+  constexpr auto kern = gemm_fp8_persistent_kernel<BN, DUAL, OutT>;
+  cudaError_t e = set_max_dynamic_smem_once<kern>(smem);
+  if (e != cudaSuccess) return e;
+  (void)launch_pdl(kern, plan.grid, dim3(kFp8Threads), smem, stream, t.w, t.w2, t.x, p, plan.tiles_n, plan.tiles_m, plan.num_tiles);
   return cudaGetLastError();
-}
-
-template <bool DUAL, typename OutT>
-cudaError_t f_dispatch_bn(int bn, const CUtensorMap& tw, const CUtensorMap& tw2, const CUtensorMap& tx, const GemmParams& p,
-                          int tiles_n, int tiles_m, int num_tiles, cudaStream_t s) {
-  switch (bn) {
-    case 16: return f_launch_one<16, DUAL, OutT>(tw, tw2, tx, p, tiles_n, tiles_m, num_tiles, s);
-    case 32: return f_launch_one<32, DUAL, OutT>(tw, tw2, tx, p, tiles_n, tiles_m, num_tiles, s);
-    case 64:
-      if constexpr (!DUAL) return f_launch_one<64, DUAL, OutT>(tw, tw2, tx, p, tiles_n, tiles_m, num_tiles, s);
-      return cudaErrorInvalidValue;
-    default: return cudaErrorInvalidValue;
-  }
 }
 
 }  // namespace
 
-cudaError_t gemm_fp8_launch(const GemmArgs& a, cudaStream_t stream) {
+cudaError_t gemm_fp8_launch(const GemmArgs& a, const GemmPlan& plan, cudaStream_t stream) {
   const bool dual = a.w2 != nullptr;
-  const bool grouped = a.expert_offsets != nullptr;
-  const int bn = std::min(a.bn > 0 ? a.bn : gemm_pick_bn(a.max_rows), dual ? kFp8MaxBNDual : kFp8MaxBN);
-  if (grouped && (a.n % kTileM) != 0) return cudaErrorInvalidValue;
+  if (a.expert_offsets != nullptr && (a.n % kTileM) != 0) return cudaErrorInvalidValue;
   if ((a.k % kFp8BlockK) != 0 || (a.n % kTileM) != 0) return cudaErrorInvalidValue;   // whole k-blocks / weight tiles only
   if (a.w_sf == nullptr || a.x_sf == nullptr || (dual && a.w2_sf == nullptr)) return cudaErrorInvalidValue;
   if (dual && a.out_fp32) return cudaErrorInvalidValue;
 
-  CUtensorMap tw, tw2, tx;
-  const uint64_t w_rows = static_cast<uint64_t>(a.n) * (grouped ? a.num_experts : 1);
-  if (!gemm_make_tmap_u8(&tw, a.w, w_rows, a.k, a.ld_w, kTileM)) return cudaErrorUnknown;
-  if (dual) {
-    if (!gemm_make_tmap_u8(&tw2, a.w2, w_rows, a.k, a.ld_w, kTileM)) return cudaErrorUnknown;
-  } else {
-    tw2 = tw;
-  }
-  if (!gemm_make_tmap_u8(&tx, a.x, a.x_rows, a.k, a.ld_x, bn)) return cudaErrorUnknown;
-
-  GemmParams p;
-  p.row_dst = nullptr; p.signal_peers = nullptr; p.num_signal_peers = 0;
-  p.m = a.m; p.n = a.n; p.k = a.k; p.splits = 1; p.cluster_splitk = 0;
-  p.expert_offsets = a.expert_offsets;
-  p.expert_stride = a.expert_stride;
+  GemmMaps t;
+  if (!gemm_maps(a, CU_TENSOR_MAP_DATA_TYPE_UINT8, plan.bn, &t)) return cudaErrorUnknown;
+  GemmParams p = gemm_params(a, plan);
   p.w_sf = static_cast<const uint32_t*>(a.w_sf); p.w2_sf = static_cast<const uint32_t*>(a.w2_sf);
   p.x_sf = static_cast<const uint32_t*>(a.x_sf); p.sf_ld_w = a.k / kFp8BlockK; p.sf_ld_x = a.k / kFp8BlockK;
-  p.out = a.out; p.ld_out = a.ld_out;
-  p.residual = static_cast<const __nv_bfloat16*>(a.residual); p.ld_res = a.ld_res;
-  p.bias = static_cast<const __nv_bfloat16*>(a.bias); p.act = a.act; p.softcap = a.softcap;
-  p.workspace = nullptr; p.tile_counters = nullptr;
-  p.signal_flag = a.signal_flag; p.signal_value = a.signal_value; p.done_counter = a.done_counter;
-  const int tiles_n = (a.n + kTileM - 1) / kTileM;
-  const int tiles_m = (a.max_rows + bn - 1) / bn;
-  const int num_tiles = tiles_n * tiles_m * (grouped ? a.num_experts : 1);
-  p.signal_tiles = a.signal_tiles > 0 ? a.signal_tiles : static_cast<unsigned int>(tiles_n * tiles_m);
   if (a.signal_peers != nullptr) {
     // EP return: every tile of the grid (empty experts included) is counted, then all peers are signalled
     p.row_dst = a.row_dst; p.signal_peers = a.signal_peers; p.num_signal_peers = a.num_signal_peers;
-    p.signal_tiles = static_cast<unsigned int>(num_tiles);
+    p.signal_tiles = static_cast<unsigned int>(plan.num_tiles);
   }
-  if (a.out_fp32) return f_dispatch_bn<false, float>(bn, tw, tw2, tx, p, tiles_n, tiles_m, num_tiles, stream);
-  if (dual) return f_dispatch_bn<true, __nv_bfloat16>(bn, tw, tw2, tx, p, tiles_n, tiles_m, num_tiles, stream);
-  return f_dispatch_bn<false, __nv_bfloat16>(bn, tw, tw2, tx, p, tiles_n, tiles_m, num_tiles, stream);
+  return dispatch_tile<kFp8MaxBN, kFp8MaxBNDual>(plan.bn, dual, a.out_fp32, [&](auto c) {
+    using C = decltype(c);
+    return f_launch_one<C::BN, C::DUAL, typename C::OutT>(t, p, plan, stream);
+  });
 }
 
 }  // namespace b200

@@ -9,8 +9,6 @@
 // accumulator tile competes with the ring (5 stages for the gate/up pair at BN = 64, 8 for a single matrix).  Token tiles are
 // loaded in 16-row boxes, only as many as the tile has valid rows: a routed expert of a decode step holds a handful of rows of its
 // 64-row segment.
-#include <algorithm>
-
 #include "gemm_common.cuh"
 #include "gemm_tmap.h"
 #include "launch.h"
@@ -322,92 +320,39 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_
 // ================================================================================================ host side
 namespace {
 
-int sm_count_cached() {
-  static int n = 0;
-  if (n == 0) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 132;
-  }
-  return n;
-}
-
 template <int BN, bool DUAL, typename OutT>
-cudaError_t p_launch_one(const CUtensorMap& tw, const CUtensorMap& tw2, const CUtensorMap& tx, const GemmParams& p, int tiles_n,
-                         int tiles_m, int num_tiles, cudaStream_t stream) {
+cudaError_t p_launch_one(const GemmMaps& t, const GemmParams& p, const GemmPlan& plan, cudaStream_t stream) {
   constexpr int STAGES = p_num_stages(BN, DUAL, sizeof(OutT));
   constexpr int smem = STAGES * stage_bytes(BN, DUAL) + p_staging_bytes(BN, sizeof(OutT)) + 2 * STAGES * 8 + 1024;
   static_assert(smem <= 227 * 1024, "shared memory budget exceeded");
-  auto kern = gemm_persistent_kernel<BN, DUAL, OutT>;
-  static bool configured = false;
-  if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) return e;
-    configured = true;
-  }
-  const int grid = std::min(num_tiles, sm_count_cached());
-  (void)launch_pdl(kern, dim3(grid), dim3(kNumThreads), smem, stream, tw, tw2, tx, p, tiles_n, tiles_m, num_tiles);
+  constexpr auto kern = gemm_persistent_kernel<BN, DUAL, OutT>;
+  cudaError_t e = set_max_dynamic_smem_once<kern>(smem);
+  if (e != cudaSuccess) return e;
+  (void)launch_pdl(kern, plan.grid, dim3(kNumThreads), smem, stream, t.w, t.w2, t.x, p, plan.tiles_n, plan.tiles_m, plan.num_tiles);
   return cudaGetLastError();
-}
-
-template <bool DUAL, typename OutT>
-cudaError_t p_dispatch_bn(int bn, const CUtensorMap& tw, const CUtensorMap& tw2, const CUtensorMap& tx, const GemmParams& p,
-                          int tiles_n, int tiles_m, int num_tiles, cudaStream_t s) {
-  switch (bn) {
-    case 16: return p_launch_one<16, DUAL, OutT>(tw, tw2, tx, p, tiles_n, tiles_m, num_tiles, s);
-    case 32: return p_launch_one<32, DUAL, OutT>(tw, tw2, tx, p, tiles_n, tiles_m, num_tiles, s);
-    case 64: return p_launch_one<64, DUAL, OutT>(tw, tw2, tx, p, tiles_n, tiles_m, num_tiles, s);
-    case 128:
-      if constexpr (!DUAL) return p_launch_one<128, DUAL, OutT>(tw, tw2, tx, p, tiles_n, tiles_m, num_tiles, s);
-      return cudaErrorInvalidValue;
-    default: return cudaErrorInvalidValue;
-  }
 }
 
 }  // namespace
 
-cudaError_t gemm_persistent_launch(const GemmArgs& a, cudaStream_t stream) {
+cudaError_t gemm_persistent_launch(const GemmArgs& a, const GemmPlan& plan, cudaStream_t stream) {
   const bool dual = a.w2 != nullptr;
-  const bool grouped = a.expert_offsets != nullptr;
-  const int bn = gemm_clamp_bn(a.bn > 0 ? a.bn : gemm_pick_bn(a.max_rows), dual);
-  if (grouped && (a.n % kTileM) != 0) return cudaErrorInvalidValue;
+  if (a.expert_offsets != nullptr && (a.n % kTileM) != 0) return cudaErrorInvalidValue;
   if ((a.k % 8) != 0 || (a.n % 8) != 0) return cudaErrorInvalidValue;
   if (dual && a.out_fp32) return cudaErrorInvalidValue;
 
-  CUtensorMap tw, tw2, tx;
-  const uint64_t w_rows = static_cast<uint64_t>(a.n) * (grouped ? a.num_experts : 1);
-  if (!gemm_make_tmap(&tw, a.w, w_rows, a.k, a.ld_w, kTileM)) return cudaErrorUnknown;
-  if (dual) {
-    if (!gemm_make_tmap(&tw2, a.w2, w_rows, a.k, a.ld_w, kTileM)) return cudaErrorUnknown;
-  } else {
-    tw2 = tw;
-  }
-  if (!gemm_make_tmap(&tx, a.x, a.x_rows, a.k, a.ld_x, kXBoxRows)) return cudaErrorUnknown;
-
-  GemmParams p;
-  p.row_dst = nullptr; p.signal_peers = nullptr; p.num_signal_peers = 0; p.w_sf = p.w2_sf = p.x_sf = nullptr; p.sf_ld_w = p.sf_ld_x = 0;
+  GemmMaps t;
+  if (!gemm_maps(a, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, kXBoxRows, &t)) return cudaErrorUnknown;
+  GemmParams p = gemm_params(a, plan);
   p.ep_arrive = a.ep_arrive; p.ep_seq = a.ep_seq; p.ep_error = a.ep_error; p.ep_world = a.ep_world; p.ep_zero_other = a.ep_zero_other ? 1 : 0;
-  p.m = a.m; p.n = a.n; p.k = a.k; p.splits = 1; p.cluster_splitk = 0;
-  p.expert_offsets = a.expert_offsets;
-  p.expert_stride = a.expert_stride;
-  p.out = a.out; p.ld_out = a.ld_out;
-  p.residual = static_cast<const __nv_bfloat16*>(a.residual); p.ld_res = a.ld_res;
-  p.bias = static_cast<const __nv_bfloat16*>(a.bias); p.act = a.act; p.softcap = a.softcap;
-  p.workspace = nullptr; p.tile_counters = nullptr;
-  p.signal_flag = a.signal_flag; p.signal_value = a.signal_value; p.done_counter = a.done_counter;
-  const int tiles_n = (a.n + kTileM - 1) / kTileM;
-  const int tiles_m = (a.max_rows + bn - 1) / bn;
-  const int num_tiles = tiles_n * tiles_m * (grouped ? a.num_experts : 1);
-  p.signal_tiles = a.signal_tiles > 0 ? a.signal_tiles : static_cast<unsigned int>(tiles_n * tiles_m);
   if (a.signal_peers != nullptr) {
     // EP return: every tile of the grid (empty experts included) is counted, then all peers are signalled
     p.row_dst = a.row_dst; p.signal_peers = a.signal_peers; p.num_signal_peers = a.num_signal_peers;
-    p.signal_tiles = static_cast<unsigned int>(num_tiles);
+    p.signal_tiles = static_cast<unsigned int>(plan.num_tiles);
   }
-  if (a.out_fp32) return p_dispatch_bn<false, float>(bn, tw, tw2, tx, p, tiles_n, tiles_m, num_tiles, stream);
-  if (dual) return p_dispatch_bn<true, __nv_bfloat16>(bn, tw, tw2, tx, p, tiles_n, tiles_m, num_tiles, stream);
-  return p_dispatch_bn<false, __nv_bfloat16>(bn, tw, tw2, tx, p, tiles_n, tiles_m, num_tiles, stream);
+  return dispatch_tile<kMaxBN, kMaxBNDual>(plan.bn, dual, a.out_fp32, [&](auto c) {
+    using C = decltype(c);
+    return p_launch_one<C::BN, C::DUAL, typename C::OutT>(t, p, plan, stream);
+  });
 }
 
 }  // namespace b200

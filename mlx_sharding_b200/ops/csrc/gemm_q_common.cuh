@@ -1,5 +1,5 @@
 // Shared pieces of the quantised (MLX affine int4/int8) wgmma GEMMs: the in-register dequantiser and the
-// cached TMA descriptor factory for packed codes / transposed scale rows.
+// TMA descriptors of packed codes / transposed scale rows.
 #pragma once
 #include "gemm_common.cuh"
 
@@ -64,9 +64,9 @@ __device__ __forceinline__ void dequant_half_row(const uint8_t* packed_row, floa
 
 }  // namespace gemm
 
-// kind 0: bf16 128B-swizzled K-major tile (activations); 1: uint32 packed codes, no swizzle; 2: bf16 row vector, no swizzle
-bool gemm_q_make_tmap(CUtensorMap* m, int kind, const void* ptr, uint64_t d0, uint64_t d1, uint64_t ld_elems, uint32_t b0, uint32_t b1);
+// Packed codes, scale and bias rows of each weight (the second set repeats the first without a pair) and the token tile.
 struct QMaps { CUtensorMap wq, wq2, s, b, s2, b2, x; };
-cudaError_t gemm_q_persistent_launch(const GemmArgs& a, cudaStream_t stream);
+bool q_maps(const GemmArgs& a, int bn, QMaps* t);
+cudaError_t gemm_q_persistent_launch(const GemmArgs& a, const GemmPlan& plan, cudaStream_t stream);
 
 }  // namespace b200

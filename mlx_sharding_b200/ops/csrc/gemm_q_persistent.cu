@@ -9,7 +9,7 @@
 //
 // HBM sees 4.5 / 8.5 bits per weight; the deep ring hides HBM latency with ~13-17 KB stages while the expensive
 // 16 KB bf16 tiles only exist DQ (2-3) at a time.
-#include <algorithm>
+#include <type_traits>
 
 #include "gemm_q_common.cuh"
 #include "launch.h"
@@ -293,98 +293,40 @@ gemm_q_persistent_kernel(const __grid_constant__ CUtensorMap tmap_wq, const __gr
 // ================================================================================================ host side
 namespace {
 
-int qp_sm_count() {
-  static int n = 0;
-  if (n == 0) {
-    int dev = 0;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&n, cudaDevAttrMultiProcessorCount, dev);
-    if (n <= 0) n = 132;
-  }
-  return n;
-}
-
 template <int BN, bool DUAL, typename OutT, int BITS>
-cudaError_t qp_launch_one(const QMaps& t, const GemmParams& p, int gk, int tiles_n, int tiles_m, int num_tiles, cudaStream_t stream) {
+cudaError_t qp_launch_one(const QMaps& t, const GemmParams& p, int gk, const GemmPlan& plan, cudaStream_t stream) {
   constexpr int STAGES = qp_num_stages(BN, DUAL, BITS, sizeof(OutT));
   constexpr int smem = qp_dq(BN, DUAL) * kATileBytes * (DUAL ? 2 : 1) + STAGES * qp_stage_bytes(BN, DUAL, BITS) + acc_bytes(BN, DUAL) +
                        qp_staging_bytes(BN, sizeof(OutT)) + (2 * STAGES + 2 * qp_dq(BN, DUAL)) * 8 + 1024;
   static_assert(smem <= 227 * 1024, "shared memory budget exceeded");
-  auto kern = gemm_q_persistent_kernel<BN, DUAL, OutT, BITS>;
-  static bool configured = false;
-  if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) return e;
-    configured = true;
-  }
-  const int grid = std::min(num_tiles, qp_sm_count());
-  (void)launch_pdl(kern, dim3(grid), dim3(kQPThreads), smem, stream, t.wq, t.wq2, t.s, t.b, t.s2, t.b2, t.x, p, gk, tiles_n, tiles_m,
-                   num_tiles);
+  constexpr auto kern = gemm_q_persistent_kernel<BN, DUAL, OutT, BITS>;
+  cudaError_t e = set_max_dynamic_smem_once<kern>(smem);
+  if (e != cudaSuccess) return e;
+  (void)launch_pdl(kern, plan.grid, dim3(kQPThreads), smem, stream, t.wq, t.wq2, t.s, t.b, t.s2, t.b2, t.x, p, gk, plan.tiles_n,
+                   plan.tiles_m, plan.num_tiles);
   return cudaGetLastError();
-}
-
-template <bool DUAL, typename OutT, int BITS>
-cudaError_t qp_dispatch_bn(int bn, const QMaps& t, const GemmParams& p, int gk, int tn, int tm, int nt, cudaStream_t s) {
-  switch (bn) {
-    case 16: return qp_launch_one<16, DUAL, OutT, BITS>(t, p, gk, tn, tm, nt, s);
-    case 32: return qp_launch_one<32, DUAL, OutT, BITS>(t, p, gk, tn, tm, nt, s);
-    case 64: return qp_launch_one<64, DUAL, OutT, BITS>(t, p, gk, tn, tm, nt, s);
-    case 128:
-      if constexpr (!DUAL) return qp_launch_one<128, DUAL, OutT, BITS>(t, p, gk, tn, tm, nt, s);
-      return cudaErrorInvalidValue;
-    default: return cudaErrorInvalidValue;
-  }
-}
-
-template <int BITS>
-cudaError_t qp_dispatch(bool dual, bool fp32, int bn, const QMaps& t, const GemmParams& p, int gk, int tn, int tm, int nt, cudaStream_t s) {
-  if (fp32) return qp_dispatch_bn<false, float, BITS>(bn, t, p, gk, tn, tm, nt, s);
-  if (dual) return qp_dispatch_bn<true, __nv_bfloat16, BITS>(bn, t, p, gk, tn, tm, nt, s);
-  return qp_dispatch_bn<false, __nv_bfloat16, BITS>(bn, t, p, gk, tn, tm, nt, s);
 }
 
 }  // namespace
 
-cudaError_t gemm_q_persistent_launch(const GemmArgs& a, cudaStream_t stream) {
+cudaError_t gemm_q_persistent_launch(const GemmArgs& a, const GemmPlan& plan, cudaStream_t stream) {
   const bool dual = a.w2 != nullptr;
-  const bool grouped = a.expert_offsets != nullptr;
-  const int bn = gemm_clamp_bn(a.bn > 0 ? a.bn : gemm_pick_bn(a.max_rows), dual);
-  if (grouped && (a.n % kTileM) != 0) return cudaErrorInvalidValue;
+  if (a.expert_offsets != nullptr && (a.n % kTileM) != 0) return cudaErrorInvalidValue;
   if ((a.n % 8) != 0 || (a.k % kBlockK) != 0) return cudaErrorInvalidValue;
   if (dual && a.out_fp32) return cudaErrorInvalidValue;
 
-  const uint64_t w_rows = static_cast<uint64_t>(a.n) * (grouped ? a.num_experts : 1);
-  const uint64_t words = static_cast<uint64_t>(a.k) * a.q_bits / 32;
-  const uint64_t ngroups = a.k / a.q_group;
   QMaps t;
-  if (!gemm_q_make_tmap(&t.wq, 1, a.w, words, w_rows, words, kBlockK * a.q_bits / 32, kTileM)) return cudaErrorUnknown;
-  if (!gemm_q_make_tmap(&t.s, 2, a.q_scales_t, w_rows, ngroups, w_rows, kTileM, 1)) return cudaErrorUnknown;
-  if (!gemm_q_make_tmap(&t.b, 2, a.q_biases_t, w_rows, ngroups, w_rows, kTileM, 1)) return cudaErrorUnknown;
-  if (dual) {
-    if (!gemm_q_make_tmap(&t.wq2, 1, a.w2, words, w_rows, words, kBlockK * a.q_bits / 32, kTileM)) return cudaErrorUnknown;
-    if (!gemm_q_make_tmap(&t.s2, 2, a.q_scales2_t, w_rows, ngroups, w_rows, kTileM, 1)) return cudaErrorUnknown;
-    if (!gemm_q_make_tmap(&t.b2, 2, a.q_biases2_t, w_rows, ngroups, w_rows, kTileM, 1)) return cudaErrorUnknown;
-  } else {
-    t.wq2 = t.wq; t.s2 = t.s; t.b2 = t.b;
-  }
-  if (!gemm_q_make_tmap(&t.x, 0, a.x, a.k, a.x_rows, a.ld_x, kBlockK, bn)) return cudaErrorUnknown;
-
-  GemmParams p;
-  p.row_dst = nullptr; p.signal_peers = nullptr; p.num_signal_peers = 0; p.w_sf = p.w2_sf = p.x_sf = nullptr; p.sf_ld_w = p.sf_ld_x = 0; p.ep_arrive = nullptr; p.ep_seq = nullptr; p.ep_error = nullptr; p.ep_world = 0; p.ep_zero_other = 0; p.expert_stride = 0;
-  p.m = a.m; p.n = a.n; p.k = a.k; p.splits = 1; p.cluster_splitk = 0;
-  p.expert_offsets = a.expert_offsets;
-  p.out = a.out; p.ld_out = a.ld_out;
-  p.residual = static_cast<const __nv_bfloat16*>(a.residual); p.ld_res = a.ld_res;
-  p.bias = static_cast<const __nv_bfloat16*>(a.bias); p.act = a.act; p.softcap = a.softcap;
-  p.workspace = nullptr; p.tile_counters = nullptr;
-  p.signal_flag = a.signal_flag; p.signal_value = a.signal_value; p.done_counter = a.done_counter;
-  const int tiles_n = (a.n + kTileM - 1) / kTileM;
-  const int tiles_m = (a.max_rows + bn - 1) / bn;
-  const int num_tiles = tiles_n * tiles_m * (grouped ? a.num_experts : 1);
-  p.signal_tiles = a.signal_tiles > 0 ? a.signal_tiles : static_cast<unsigned int>(tiles_n * tiles_m);
+  if (!q_maps(a, plan.bn, &t)) return cudaErrorUnknown;
+  const GemmParams p = gemm_params(a, plan);
   const int gk = a.q_group / kBlockK;
-  if (a.q_bits == 4) return qp_dispatch<4>(dual, a.out_fp32, bn, t, p, gk, tiles_n, tiles_m, num_tiles, stream);
-  return qp_dispatch<8>(dual, a.out_fp32, bn, t, p, gk, tiles_n, tiles_m, num_tiles, stream);
+  auto dispatch = [&](auto bits) {
+    return dispatch_tile<kMaxBN, kMaxBNDual>(plan.bn, dual, a.out_fp32, [&](auto c) {
+      using C = decltype(c);
+      return qp_launch_one<C::BN, C::DUAL, typename C::OutT, decltype(bits)::value>(t, p, gk, plan, stream);
+    });
+  };
+  if (a.q_bits == 4) return dispatch(std::integral_constant<int, 4>{});
+  return dispatch(std::integral_constant<int, 8>{});
 }
 
 }  // namespace b200

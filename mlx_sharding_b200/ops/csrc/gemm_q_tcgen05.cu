@@ -10,10 +10,10 @@
 //   MMA warpgroup: wgmma (fp32 accumulators in registers), wait                        -> empty barrier
 // so HBM only ever sees 4.5 (or 8.5) bits per weight; everything downstream (epilogue, DUAL gate/up,
 // grouped experts, split-K, fused P2P signal) is shared with the dense kernel (gemm_common.cuh).
-#include <mutex>
-#include <unordered_map>
+#include <type_traits>
 
 #include "gemm_q_common.cuh"
+#include "gemm_tmap.h"
 #include "launch.h"
 
 namespace b200 {
@@ -174,153 +174,73 @@ gemm_swapab_q_kernel(const __grid_constant__ CUtensorMap tmap_wq, const __grid_c
 // ================================================================================================ host side
 namespace {
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeTiledFn q_encode_fn() {
-  static EncodeTiledFn fn = nullptr;
-  if (fn == nullptr) {
-    void* ptr = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) != cudaSuccess ||
-        qres != cudaDriverEntryPointSuccess)
-      return nullptr;
-    fn = reinterpret_cast<EncodeTiledFn>(ptr);
-  }
-  return fn;
-}
-
-struct QKey {
-  const void* ptr; uint64_t d0, d1, ld; uint32_t b0, b1; int kind;
-  bool operator==(const QKey& o) const { return ptr == o.ptr && d0 == o.d0 && d1 == o.d1 && ld == o.ld && b0 == o.b0 && b1 == o.b1 && kind == o.kind; }
-};
-struct QKeyHash {
-  size_t operator()(const QKey& k) const {
-    size_t h = std::hash<const void*>()(k.ptr);
-    h ^= std::hash<uint64_t>()(k.d0 * 1000003ull + k.d1 * 7919ull + k.ld) + 0x9e3779b97f4a7c15ull + (h << 6) + (h >> 2);
-    h ^= std::hash<uint64_t>()(((uint64_t)k.b0 << 32) | (k.b1 * 8u + k.kind)) + 0x9e3779b97f4a7c15ull + (h << 6) + (h >> 2);
-    return h;
-  }
-};
-std::unordered_map<QKey, CUtensorMap, QKeyHash> g_qcache;
-std::mutex g_qmutex;
-
-// kind 0: bf16 128B-swizzled K-major tile (activations); 1: uint32 packed codes, no swizzle; 2: bf16 row vector, no swizzle
-bool q_make_tmap(CUtensorMap* m, int kind, const void* ptr, uint64_t d0, uint64_t d1, uint64_t ld_elems, uint32_t b0, uint32_t b1) {
-  const QKey key{ptr, d0, d1, ld_elems, b0, b1, kind};
-  std::lock_guard<std::mutex> lock(g_qmutex);
-  auto it = g_qcache.find(key);
-  if (it != g_qcache.end()) { *m = it->second; return true; }
-  EncodeTiledFn fn = q_encode_fn();
-  if (fn == nullptr) return false;
-  const uint32_t esz = kind == 1 ? 4 : 2;
-  cuuint64_t dims[2] = {d0, d1};
-  cuuint64_t strides[1] = {ld_elems * esz};
-  cuuint32_t box[2] = {b0, b1};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = fn(m, kind == 1 ? CU_TENSOR_MAP_DATA_TYPE_UINT32 : CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims,
-                  strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE, kind == 0 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE,
-                  CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r != CUDA_SUCCESS) return false;
-  if (g_qcache.size() > 16384) g_qcache.clear();
-  g_qcache.emplace(key, *m);
-  return true;
-}
-
-
 template <int BN, bool DUAL, typename OutT, int BITS>
-cudaError_t q_launch_one(const QMaps& t, const GemmParams& p, int group_kblocks, dim3 grid, cudaStream_t stream) {
+cudaError_t q_launch_one(const QMaps& t, const GemmParams& p, int group_kblocks, const GemmPlan& plan, cudaStream_t stream) {
   constexpr int STAGES = q_num_stages(BN, DUAL, BITS, sizeof(OutT));
   constexpr int smem = STAGES * q_stage_bytes(BN, DUAL, BITS) + 3 * STAGES * 8 + 16 + 1024;
   static_assert(smem <= 227 * 1024, "shared memory budget exceeded");
-  auto kern = gemm_swapab_q_kernel<BN, DUAL, OutT, BITS>;
-  static bool configured = false;
-  if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) return e;
-    configured = true;
-  }
-  (void)launch_pdl(kern, dim3(grid), dim3(kQThreads), smem, stream, t.wq, t.wq2, t.s, t.b, t.s2, t.b2, t.x, p, group_kblocks);
+  constexpr auto kern = gemm_swapab_q_kernel<BN, DUAL, OutT, BITS>;
+  cudaError_t e = set_max_dynamic_smem_once<kern>(smem);
+  if (e != cudaSuccess) return e;
+  (void)launch_pdl(kern, plan.grid, dim3(kQThreads), smem, stream, t.wq, t.wq2, t.s, t.b, t.s2, t.b2, t.x, p, group_kblocks);
   return cudaGetLastError();
-}
-
-template <bool DUAL, typename OutT, int BITS>
-cudaError_t q_dispatch_bn(int bn, const QMaps& t, const GemmParams& p, int gk, dim3 grid, cudaStream_t s) {
-  switch (bn) {
-    case 16: return q_launch_one<16, DUAL, OutT, BITS>(t, p, gk, grid, s);
-    case 32: return q_launch_one<32, DUAL, OutT, BITS>(t, p, gk, grid, s);
-    case 64: return q_launch_one<64, DUAL, OutT, BITS>(t, p, gk, grid, s);
-    case 128:
-      if constexpr (!DUAL) return q_launch_one<128, DUAL, OutT, BITS>(t, p, gk, grid, s);
-      return cudaErrorInvalidValue;
-    default: return cudaErrorInvalidValue;
-  }
-}
-
-template <int BITS>
-cudaError_t q_dispatch(bool dual, bool fp32, int bn, const QMaps& t, const GemmParams& p, int gk, dim3 grid, cudaStream_t s) {
-  if (fp32) return q_dispatch_bn<false, float, BITS>(bn, t, p, gk, grid, s);
-  if (dual) return q_dispatch_bn<true, __nv_bfloat16, BITS>(bn, t, p, gk, grid, s);
-  return q_dispatch_bn<false, __nv_bfloat16, BITS>(bn, t, p, gk, grid, s);
 }
 
 }  // namespace
 
-bool gemm_q_make_tmap(CUtensorMap* m, int kind, const void* ptr, uint64_t d0, uint64_t d1, uint64_t ld_elems, uint32_t b0, uint32_t b1) {
-  return q_make_tmap(m, kind, ptr, d0, d1, ld_elems, b0, b1);
+bool q_maps(const GemmArgs& a, int bn, QMaps* t) {
+  const uint64_t w_rows = static_cast<uint64_t>(a.n) * (a.expert_offsets != nullptr ? a.num_experts : 1);
+  const uint64_t words = static_cast<uint64_t>(a.k) * a.q_bits / 32;
+  // packed codes: uint32 [w_rows, words] in unswizzled boxes of 128 rows x one k-block
+  auto codes = [&](CUtensorMap* m, const void* ptr) {
+    TmapSpec s;
+    s.ptr = ptr; s.dtype = CU_TENSOR_MAP_DATA_TYPE_UINT32; s.swizzle = CU_TENSOR_MAP_SWIZZLE_NONE;
+    s.dims[0] = words; s.dims[1] = w_rows; s.strides[0] = words * 4;
+    s.box[0] = kBlockK * a.q_bits / 32; s.box[1] = kTileM;
+    return tmap_cached(m, s);
+  };
+  // scales / biases: bf16 [k / group, w_rows] in unswizzled boxes of 128 rows of one group
+  auto group_rows = [&](CUtensorMap* m, const void* ptr) {
+    TmapSpec s;
+    s.ptr = ptr; s.swizzle = CU_TENSOR_MAP_SWIZZLE_NONE;
+    s.dims[0] = w_rows; s.dims[1] = a.k / a.q_group; s.strides[0] = w_rows * 2;
+    s.box[0] = kTileM; s.box[1] = 1;
+    return tmap_cached(m, s);
+  };
+  if (!codes(&t->wq, a.w) || !group_rows(&t->s, a.q_scales_t) || !group_rows(&t->b, a.q_biases_t)) return false;
+  if (a.w2 != nullptr) {
+    if (!codes(&t->wq2, a.w2) || !group_rows(&t->s2, a.q_scales2_t) || !group_rows(&t->b2, a.q_biases2_t)) return false;
+  } else {
+    t->wq2 = t->wq; t->s2 = t->s; t->b2 = t->b;
+  }
+  return gemm_tmap(&t->x, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, a.x, a.x_rows, a.k, a.ld_x, bn);
 }
 
 bool gemm_q_supported(int bits, int group, int k) {
   return (bits == 4 || bits == 8) && (group == 64 || group == 128) && (k % 64) == 0 && (k % group) == 0;
 }
 
-cudaError_t gemm_q_launch(const GemmArgs& a, cudaStream_t stream) {
+cudaError_t gemm_q_launch(const GemmArgs& a, const GemmPlan& plan, cudaStream_t stream) {
   if (!gemm_q_supported(a.q_bits, a.q_group, a.k)) return cudaErrorNotSupported;
+  if (plan.route == kRoutePersistent) return gemm_q_persistent_launch(a, plan, stream);
   const bool dual = a.w2 != nullptr;
-  const bool grouped = a.expert_offsets != nullptr;
-  const int bn = gemm_clamp_bn(a.bn > 0 ? a.bn : gemm_pick_bn(a.max_rows), dual);
-  int splits = a.splits > 0 ? a.splits : 1;
-  if (splits == 1 && a.persistent) return gemm_q_persistent_launch(a, stream);
-  const int kb_total = a.k / kBlockK;
-  if (splits > kb_total) splits = kb_total;
-  if (grouped && (a.n % kTileM) != 0) return cudaErrorInvalidValue;
+  if (a.expert_offsets != nullptr && (a.n % kTileM) != 0) return cudaErrorInvalidValue;
   if ((a.n % 8) != 0) return cudaErrorInvalidValue;
-  if (splits > 1 && (a.workspace == nullptr || a.tile_counters == nullptr)) return cudaErrorInvalidValue;
+  if (a.workspace == nullptr || a.tile_counters == nullptr) return cudaErrorInvalidValue;
   if (dual && a.out_fp32) return cudaErrorInvalidValue;
 
-  const uint64_t w_rows = static_cast<uint64_t>(a.n) * (grouped ? a.num_experts : 1);
-  const uint64_t words = static_cast<uint64_t>(a.k) * a.q_bits / 32;
-  const uint64_t ngroups = a.k / a.q_group;
   QMaps t;
-  if (!q_make_tmap(&t.wq, 1, a.w, words, w_rows, words, kBlockK * a.q_bits / 32, kTileM)) return cudaErrorUnknown;
-  if (!q_make_tmap(&t.s, 2, a.q_scales_t, w_rows, ngroups, w_rows, kTileM, 1)) return cudaErrorUnknown;
-  if (!q_make_tmap(&t.b, 2, a.q_biases_t, w_rows, ngroups, w_rows, kTileM, 1)) return cudaErrorUnknown;
-  if (dual) {
-    if (!q_make_tmap(&t.wq2, 1, a.w2, words, w_rows, words, kBlockK * a.q_bits / 32, kTileM)) return cudaErrorUnknown;
-    if (!q_make_tmap(&t.s2, 2, a.q_scales2_t, w_rows, ngroups, w_rows, kTileM, 1)) return cudaErrorUnknown;
-    if (!q_make_tmap(&t.b2, 2, a.q_biases2_t, w_rows, ngroups, w_rows, kTileM, 1)) return cudaErrorUnknown;
-  } else {
-    t.wq2 = t.wq; t.s2 = t.s; t.b2 = t.b;
-  }
-  if (!q_make_tmap(&t.x, 0, a.x, a.k, a.x_rows, a.ld_x, kBlockK, bn)) return cudaErrorUnknown;
-
-  GemmParams p;
-  p.row_dst = nullptr; p.signal_peers = nullptr; p.num_signal_peers = 0; p.w_sf = p.w2_sf = p.x_sf = nullptr; p.sf_ld_w = p.sf_ld_x = 0; p.ep_arrive = nullptr; p.ep_seq = nullptr; p.ep_error = nullptr; p.ep_world = 0; p.ep_zero_other = 0; p.expert_stride = 0;
-  p.m = a.m; p.n = a.n; p.k = a.k; p.splits = splits;
-  p.cluster_splitk = 0;
-  p.expert_offsets = a.expert_offsets;
-  p.out = a.out; p.ld_out = a.ld_out;
-  p.residual = static_cast<const __nv_bfloat16*>(a.residual); p.ld_res = a.ld_res;
-  p.bias = static_cast<const __nv_bfloat16*>(a.bias); p.act = a.act; p.softcap = a.softcap;
-  p.workspace = a.workspace; p.tile_counters = a.tile_counters;
-  p.signal_flag = a.signal_flag; p.signal_value = a.signal_value; p.done_counter = a.done_counter;
-  const int tiles_n = (a.n + kTileM - 1) / kTileM;
-  const int tiles_m = (a.max_rows + bn - 1) / bn;
-  dim3 grid(tiles_n, grouped ? a.num_experts : 1, tiles_m * splits);
-  p.signal_tiles = a.signal_tiles > 0 ? a.signal_tiles : static_cast<unsigned int>(tiles_n * tiles_m);
+  if (!q_maps(a, plan.bn, &t)) return cudaErrorUnknown;
+  const GemmParams p = gemm_params(a, plan);
   const int gk = a.q_group / kBlockK;  // k-blocks per quantisation group (1 or 2)
-  if (a.q_bits == 4) return q_dispatch<4>(dual, a.out_fp32, bn, t, p, gk, grid, stream);
-  return q_dispatch<8>(dual, a.out_fp32, bn, t, p, gk, grid, stream);
+  auto dispatch = [&](auto bits) {
+    return dispatch_tile<kMaxBN, kMaxBNDual>(plan.bn, dual, a.out_fp32, [&](auto c) {
+      using C = decltype(c);
+      return q_launch_one<C::BN, C::DUAL, typename C::OutT, decltype(bits)::value>(t, p, gk, plan, stream);
+    });
+  };
+  if (a.q_bits == 4) return dispatch(std::integral_constant<int, 4>{});
+  return dispatch(std::integral_constant<int, 8>{});
 }
 
 }  // namespace b200

@@ -23,10 +23,6 @@
 //    after a system-scope fence — GEMM + P2P hand-off in one kernel, no NCCL call, no host hop.
 #include "gemm_tcgen05.h"
 
-#include <algorithm>
-#include <mutex>
-#include <unordered_map>
-
 #include "gemm_cluster.cuh"
 #include "gemm_tmap.h"
 #include "launch.h"
@@ -165,185 +161,35 @@ gemm_swapab_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_cons
 // ================================================================================================ host side
 namespace {
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-
-EncodeTiledFn get_encode_fn() {
-  static EncodeTiledFn fn = nullptr;
-  if (fn == nullptr) {
-    void* ptr = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    cudaError_t e = cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres);
-    if (e != cudaSuccess || qres != cudaDriverEntryPointSuccess || ptr == nullptr) return nullptr;
-    fn = reinterpret_cast<EncodeTiledFn>(ptr);
-  }
-  return fn;
-}
-
-// Descriptor cache: encoding a tensor map costs a few microseconds of host time; weights (and the static
-// activation buffers of graph-captured steps) are encoded once.
-struct TmapKey {
-  const void* ptr; uint64_t rows, cols, ld; uint32_t box;
-  bool operator==(const TmapKey& o) const { return ptr == o.ptr && rows == o.rows && cols == o.cols && ld == o.ld && box == o.box; }
-};
-struct TmapKeyHash {
-  size_t operator()(const TmapKey& k) const {
-    size_t h = std::hash<const void*>()(k.ptr);
-    h ^= std::hash<uint64_t>()(k.rows * 1000003ull + k.cols) + 0x9e3779b97f4a7c15ull + (h << 6) + (h >> 2);
-    h ^= std::hash<uint64_t>()(k.ld * 31ull + k.box) + 0x9e3779b97f4a7c15ull + (h << 6) + (h >> 2);
-    return h;
-  }
-};
-std::unordered_map<TmapKey, CUtensorMap, TmapKeyHash> g_tmap_cache;
-std::mutex g_tmap_mutex;
-
-bool encode_tmap(CUtensorMap* m, const void* ptr, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows);
-
-// bf16 row-major [rows, cols] (row stride ld elements) -> tiles of box_rows x 64 with 128B swizzle
-bool make_tmap(CUtensorMap* m, const void* ptr, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows) {
-  const TmapKey key{ptr, rows, cols, ld, box_rows};
-  std::lock_guard<std::mutex> lock(g_tmap_mutex);
-  auto it = g_tmap_cache.find(key);
-  if (it != g_tmap_cache.end()) { *m = it->second; return true; }
-  if (!encode_tmap(m, ptr, rows, cols, ld, box_rows)) return false;
-  if (g_tmap_cache.size() > 16384) g_tmap_cache.clear();
-  g_tmap_cache.emplace(key, *m);
-  return true;
-}
-
-bool encode_tmap(CUtensorMap* m, const void* ptr, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows) {
-  EncodeTiledFn fn = get_encode_fn();
-  if (fn == nullptr) return false;
-  cuuint64_t dims[2] = {cols, rows};
-  cuuint64_t strides[1] = {ld * 2};
-  cuuint32_t box[2] = {kBlockK, box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  CUresult r = fn(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, estr,
-                  CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                  CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  return r == CUDA_SUCCESS;
-}
-
 template <int BN, bool DUAL, typename OutT>
-cudaError_t launch_one(const GemmArgs& a, const CUtensorMap& tw, const CUtensorMap& tw2, const CUtensorMap& tx,
-                       const GemmParams& p, dim3 grid, cudaStream_t stream) {
+cudaError_t launch_one(const GemmMaps& t, const GemmParams& p, const GemmPlan& plan, cudaStream_t stream) {
   constexpr int STAGES = num_stages(BN, DUAL, sizeof(OutT));
   constexpr int smem = STAGES * stage_bytes(BN, DUAL) + 2 * STAGES * 8 + 16 + 1024;
   static_assert(smem <= 227 * 1024, "shared memory budget exceeded");
-  auto kern = gemm_swapab_kernel<BN, DUAL, OutT>;
-  static bool configured = false;
-  if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) return e;
-    configured = true;
-  }
-  (void)launch_pdl_cluster(kern, dim3(grid), dim3(kNumThreads), smem, stream, p.cluster_splitk ? (unsigned)p.splits : 1u, tw, tw2, tx, p);
+  constexpr auto kern = gemm_swapab_kernel<BN, DUAL, OutT>;
+  cudaError_t e = set_max_dynamic_smem_once<kern>(smem);
+  if (e != cudaSuccess) return e;
+  (void)launch_pdl_cluster(kern, plan.grid, dim3(kNumThreads), smem, stream, plan.cluster_z, t.w, t.w2, t.x, p);
   return cudaGetLastError();
-}
-
-template <bool DUAL, typename OutT>
-cudaError_t dispatch_bn(int bn, const GemmArgs& a, const CUtensorMap& tw, const CUtensorMap& tw2, const CUtensorMap& tx,
-                        const GemmParams& p, dim3 grid, cudaStream_t s) {
-  switch (bn) {
-    case 16: return launch_one<16, DUAL, OutT>(a, tw, tw2, tx, p, grid, s);
-    case 32: return launch_one<32, DUAL, OutT>(a, tw, tw2, tx, p, grid, s);
-    case 64: return launch_one<64, DUAL, OutT>(a, tw, tw2, tx, p, grid, s);
-    case 128:
-      if constexpr (!DUAL) return launch_one<128, DUAL, OutT>(a, tw, tw2, tx, p, grid, s);
-      return cudaErrorInvalidValue;
-    default: return cudaErrorInvalidValue;
-  }
 }
 
 }  // namespace
 
-bool gemm_make_tmap(CUtensorMap* m, const void* ptr, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows) {
-  return make_tmap(m, ptr, rows, cols, ld, box_rows);
-}
-
-bool gemm_make_tmap_u8(CUtensorMap* m, const void* ptr, uint64_t rows, uint64_t cols, uint64_t ld, uint32_t box_rows) {
-  // same cache, keyed with the top bit of the box to keep bf16 and byte maps of one pointer apart
-  const TmapKey key{ptr, rows, cols, ld, box_rows | 0x80000000u};
-  std::lock_guard<std::mutex> lock(g_tmap_mutex);
-  auto it = g_tmap_cache.find(key);
-  if (it != g_tmap_cache.end()) { *m = it->second; return true; }
-  EncodeTiledFn fn = get_encode_fn();
-  if (fn == nullptr) return false;
-  cuuint64_t dims[2] = {cols, rows};
-  cuuint64_t strides[1] = {ld};
-  cuuint32_t box[2] = {128, box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  if (fn(m, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-         CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-    return false;
-  if (g_tmap_cache.size() > 16384) g_tmap_cache.clear();
-  g_tmap_cache.emplace(key, *m);
-  return true;
-}
-
-int gemm_pick_bn(int max_rows) {
-  if (max_rows <= 16) return 16;
-  if (max_rows <= 32) return 32;
-  if (max_rows <= 64) return 64;
-  return kMaxBN;
-}
-
-int gemm_clamp_bn(int bn, bool dual) { return std::min(bn, dual ? kMaxBNDual : kMaxBN); }
-
-size_t gemm_workspace_floats(const GemmArgs& a, int bn, int splits) {
-  if (splits <= 1) return 0;
-  const size_t tiles_n = (a.n + kTileM - 1) / kTileM;
-  const size_t tiles_m = (a.max_rows + bn - 1) / bn;
-  return tiles_n * (a.num_experts > 0 ? a.num_experts : 1) * tiles_m * splits * (size_t)bn * (a.w2 ? 2 : 1) * kTileM;
-}
-
-cudaError_t gemm_launch(const GemmArgs& a, cudaStream_t stream) {
+cudaError_t gemm_launch(const GemmArgs& a, const GemmPlan& plan, cudaStream_t stream) {
+  if (plan.route == kRoutePersistent) return gemm_persistent_launch(a, plan, stream);
   const bool dual = a.w2 != nullptr;
-  const bool grouped = a.expert_offsets != nullptr;
-  const int bn = gemm_clamp_bn(a.bn > 0 ? a.bn : gemm_pick_bn(a.max_rows), dual);
-  int splits = a.splits > 0 ? a.splits : 1;
-  const int kb_total = (a.k + kBlockK - 1) / kBlockK;
-  if (splits > kb_total) splits = kb_total;
-  if (splits == 1 && a.persistent) return gemm_persistent_launch(a, stream);  // no split-K: persistent tile loop
-  if (grouped && (a.n % kTileM) != 0) return cudaErrorInvalidValue;
+  if (a.expert_offsets != nullptr && (a.n % kTileM) != 0) return cudaErrorInvalidValue;
   if ((a.k % 8) != 0 || (a.n % 8) != 0) return cudaErrorInvalidValue;
-  if (splits > 1 && !a.cluster_splitk && (a.workspace == nullptr || a.tile_counters == nullptr)) return cudaErrorInvalidValue;
+  if (plan.route == kRouteWorkspaceSplitK && (a.workspace == nullptr || a.tile_counters == nullptr)) return cudaErrorInvalidValue;
   if (dual && a.out_fp32) return cudaErrorInvalidValue;
 
-  CUtensorMap tw, tw2, tx;
-  const uint64_t w_rows = static_cast<uint64_t>(a.n) * (grouped ? a.num_experts : 1);
-  if (!make_tmap(&tw, a.w, w_rows, a.k, a.ld_w, kTileM)) return cudaErrorUnknown;
-  if (dual) {
-    if (!make_tmap(&tw2, a.w2, w_rows, a.k, a.ld_w, kTileM)) return cudaErrorUnknown;
-  } else {
-    tw2 = tw;
-  }
-  if (!make_tmap(&tx, a.x, a.x_rows, a.k, a.ld_x, bn)) return cudaErrorUnknown;
-
-  GemmParams p;
-  p.row_dst = nullptr; p.signal_peers = nullptr; p.num_signal_peers = 0; p.w_sf = p.w2_sf = p.x_sf = nullptr; p.sf_ld_w = p.sf_ld_x = 0; p.ep_arrive = nullptr; p.ep_seq = nullptr; p.ep_error = nullptr; p.ep_world = 0; p.ep_zero_other = 0;
-  p.m = a.m; p.n = a.n; p.k = a.k; p.splits = splits;
-  // DSMEM (cluster) split-K when the fp32 partial tile fits the idle stage ring and the cluster is portable
-  p.cluster_splitk = (a.cluster_splitk && splits > 1 && splits <= 8 && bn * (dual ? 2 : 1) <= 128) ? 1 : 0;
-  p.expert_offsets = a.expert_offsets;
-  p.expert_stride = a.expert_stride;
-  p.out = a.out; p.ld_out = a.ld_out;
-  p.residual = static_cast<const __nv_bfloat16*>(a.residual); p.ld_res = a.ld_res;
-  p.bias = static_cast<const __nv_bfloat16*>(a.bias); p.act = a.act; p.softcap = a.softcap;
-  p.workspace = a.workspace; p.tile_counters = a.tile_counters;
-  p.signal_flag = a.signal_flag; p.signal_value = a.signal_value; p.done_counter = a.done_counter;
-
-  const int tiles_n = (a.n + kTileM - 1) / kTileM;
-  const int tiles_m = (a.max_rows + bn - 1) / bn;
-  dim3 grid(tiles_n, grouped ? a.num_experts : 1, tiles_m * splits);
-  // tiles that run the epilogue (= tiles that will tick done_counter); for grouped launches the caller
-  // passes the exact count (empty experts exit early)
-  p.signal_tiles = a.signal_tiles > 0 ? a.signal_tiles : static_cast<unsigned int>(tiles_n * tiles_m);
-
-  if (a.out_fp32) return dispatch_bn<false, float>(bn, a, tw, tw2, tx, p, grid, stream);
-  if (dual) return dispatch_bn<true, __nv_bfloat16>(bn, a, tw, tw2, tx, p, grid, stream);
-  return dispatch_bn<false, __nv_bfloat16>(bn, a, tw, tw2, tx, p, grid, stream);
+  GemmMaps t;
+  if (!gemm_maps(a, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, plan.bn, &t)) return cudaErrorUnknown;
+  const GemmParams p = gemm_params(a, plan);
+  return dispatch_tile<kMaxBN, kMaxBNDual>(plan.bn, dual, a.out_fp32, [&](auto c) {
+    using C = decltype(c);
+    return launch_one<C::BN, C::DUAL, typename C::OutT>(t, p, plan, stream);
+  });
 }
 
 }  // namespace b200

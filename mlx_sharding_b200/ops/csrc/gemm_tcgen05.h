@@ -50,7 +50,8 @@ struct GemmArgs {
   int m = 0;                      // rows when not grouped
   int n = 0, k = 0;
   int max_rows = 0;               // upper bound of rows per (expert) problem: sizes the grid
-  int num_experts = 0;            // grouped: number of experts
+  int num_experts = 0;            // grouped: number of experts (0: dense)
+  long long expected_rows = 0;    // grouped: rows expected over all experts, sizes the token tile (0: sized for max_rows)
   const int* expert_offsets = nullptr;  // grouped: int32 [num_experts + 1] row offsets into x / out (device)
   const unsigned long long* ep_arrive = nullptr; const uint32_t* ep_seq = nullptr; uint32_t* ep_error = nullptr;
   int ep_world = 0; bool ep_zero_other = false;   // EP receive side: arrival wait fused into the grouped GEMM (see GemmParams)
@@ -63,14 +64,12 @@ struct GemmArgs {
   const void* bias = nullptr;     // bf16 [n]
   int act = kActNone;             // used with w2
   float softcap = 0.f;            // y = cap * tanh(y / cap) (Gemma-2 final logits)
-  int bn = 0;                     // token tile (0 = auto)
-  int splits = 1;                 // split-K factor
-  float* workspace = nullptr;     // fp32, gemm_workspace_floats() elements when splits > 1
-  unsigned int* tile_counters = nullptr;  // zero-initialised, >= number of output tiles
+  int splits = 0;                 // split-K factor (0 = chosen by gemm_plan)
+  float* workspace = nullptr;     // fp32, GemmPlan::workspace_floats elements (workspace split-K route only)
+  unsigned int* tile_counters = nullptr;  // zero-initialised, >= number of output tiles (workspace split-K route only)
   uint32_t* signal_flag = nullptr;        // fused stage boundary: raised (release.sys) when every tile is stored
   uint32_t signal_value = 0;
   unsigned int* done_counter = nullptr;   // zero-initialised device counter
-  unsigned int signal_tiles = 0;          // 0 = all tiles of the grid
   const unsigned long long* row_dst = nullptr;       // EP return: per-row destination addresses (device array)
   const unsigned long long* signal_peers = nullptr;  // EP return: device table of peer flag addresses
   int num_signal_peers = 0;
@@ -78,20 +77,41 @@ struct GemmArgs {
   // scales / biases are pre-transposed to [k/group, rows] bf16 at load time (TMA-friendly)
   // block-scaled FP8 (gemm_fp8_launch): w / w2 / x point at e4m3 bytes, *_sf at their ue8m0 scales [rows, k / 32]
   const void* w_sf = nullptr; const void* w2_sf = nullptr; const void* x_sf = nullptr;
-  bool persistent = true;                 // splits == 1: persistent kernel (gemm_persistent.cu)
-  bool cluster_splitk = true;             // prefer the DSMEM reduction when it applies (decode shapes)
   int q_bits = 0, q_group = 64;
   const void* q_scales_t = nullptr; const void* q_biases_t = nullptr;
   const void* q_scales2_t = nullptr; const void* q_biases2_t = nullptr;
 };
 
-int gemm_pick_bn(int max_rows);
-int gemm_clamp_bn(int bn, bool dual);  // largest token tile the register accumulators allow
-size_t gemm_workspace_floats(const GemmArgs& a, int bn, int splits);
-cudaError_t gemm_launch(const GemmArgs& a, cudaStream_t stream);
-cudaError_t gemm_persistent_launch(const GemmArgs& a, cudaStream_t stream);
+// Weight format of a launch: bf16, MLX affine int4 / int8 (dequantised in the kernel), MXFP8.
+enum GemmKind : int { kGemmBf16 = 0, kGemmQuant = 1, kGemmFp8 = 2 };
+
+enum GemmRoute : int {
+  kRoutePersistent = 0,       // no split-K: one CTA per SM walks the tile list (gemm_persistent.cu, gemm_q_persistent.cu, gemm_fp8.cu)
+  kRouteClusterSplitK = 1,    // the `splits` CTAs of a tile form a cluster and reduce through DSMEM (bf16 only)
+  kRouteWorkspaceSplitK = 2,  // partial tiles go through an fp32 workspace, the last CTA of a tile reduces them
+};
+
+// Every host-side choice of a launch, made once by gemm_plan and read by the binding (workspace) and the launcher.
+struct GemmPlan {
+  GemmRoute route = kRoutePersistent;
+  int bn = 0;                  // token tile
+  int splits = 1;              // split-K factor, <= the k-block count
+  int tiles_n = 0, tiles_m = 0, num_tiles = 0;  // 128-feature tiles, token tiles per expert, tiles of all experts
+  dim3 grid;
+  unsigned cluster_z = 1;      // CTAs per cluster along z
+  size_t workspace_floats = 0;  // fp32 workspace the route reads
+};
+
+// Pure function of the launch shape (rows, n, k, pair, experts, expected rows, requested splits) and the SM count.
+GemmPlan gemm_plan(const GemmArgs& a, GemmKind kind, int sm_count);
+// Kernel parameters shared by every route: zero-initialised, then the launch's common fields and the plan's split-K choice.
+GemmParams gemm_params(const GemmArgs& a, const GemmPlan& plan);
+int sm_count();  // of the current device, read once
+
+cudaError_t gemm_launch(const GemmArgs& a, const GemmPlan& plan, cudaStream_t stream);
+cudaError_t gemm_persistent_launch(const GemmArgs& a, const GemmPlan& plan, cudaStream_t stream);
 bool gemm_q_supported(int bits, int group, int k);
-cudaError_t gemm_q_launch(const GemmArgs& a, cudaStream_t stream);
-cudaError_t gemm_fp8_launch(const GemmArgs& a, cudaStream_t stream);   // MXFP8 x MXFP8 -> bf16 / fp32 (gemm_fp8.cu)
+cudaError_t gemm_q_launch(const GemmArgs& a, const GemmPlan& plan, cudaStream_t stream);
+cudaError_t gemm_fp8_launch(const GemmArgs& a, const GemmPlan& plan, cudaStream_t stream);   // MXFP8 x MXFP8 -> bf16 / fp32 (gemm_fp8.cu)
 
 }  // namespace b200

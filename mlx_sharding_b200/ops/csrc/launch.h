@@ -45,11 +45,18 @@ inline cudaError_t launch_pdl(void (*kernel)(KArgs...), dim3 grid, dim3 block, s
   return cudaLaunchKernelEx(&cfg, kernel, static_cast<KArgs>(args)...);
 }
 
-}  // namespace b200
+// Raises the dynamic shared memory limit of `Kernel` to `bytes` on its first launch.  One flag per kernel instance; a failed
+// attempt is not remembered, so the next launch tries again.
+template <auto Kernel>
+inline cudaError_t set_max_dynamic_smem_once(int bytes) {
+  static bool configured = false;
+  if (configured) return cudaSuccess;
+  const cudaError_t e = cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+  configured = e == cudaSuccess;
+  return e;
+}
 
-namespace b200 {
-
-// Same, with a thread-block cluster of {1, 1, cluster_z} CTAs (DSMEM split-K reduction).
+// Same as launch_pdl, with a thread-block cluster of {1, 1, cluster_z} CTAs (DSMEM split-K reduction).
 template <typename... KArgs, typename... Args>
 inline cudaError_t launch_pdl_cluster(void (*kernel)(KArgs...), dim3 grid, dim3 block, size_t smem, cudaStream_t stream,
                                       unsigned cluster_z, Args&&... args) {

@@ -23,6 +23,7 @@
 // Decode only (one query token per sequence); prefill chunks take the decompressing path (models/deepseek_v2.py).
 #include <cuda.h>
 
+#include "gemm_tmap.h"
 #include "kernels.h"
 #include "launch.h"
 #include "ptx.cuh"
@@ -360,22 +361,6 @@ mla_absorbed_prologue_kernel(__nv_bfloat16* __restrict__ q, long long q_ld_t, co
   }
 }
 
-typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
-                                  const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
-                                  CUtensorMapL2promotion, CUtensorMapFloatOOBfill);
-EncodeTiledFn encode_fn() {
-  static EncodeTiledFn fn = nullptr;
-  if (fn == nullptr) {
-    void* ptr = nullptr;
-    cudaDriverEntryPointQueryResult qres;
-    if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) != cudaSuccess ||
-        qres != cudaDriverEntryPointSuccess)
-      return nullptr;
-    fn = reinterpret_cast<EncodeTiledFn>(ptr);
-  }
-  return fn;
-}
-
 }  // namespace
 
 cudaError_t mla_absorbed_prologue_launch(void* q, long long q_ld_t, const void* ckv, long long ckv_ld_t, const void* kpe,
@@ -398,28 +383,20 @@ cudaError_t mla_decode_launch(const void* q, long long q_ld_t, int B, const void
                               int nsplit, float* workspace, void* out, long long o_ld_t, long long* dbg, cudaStream_t s) {
   if (B == 0) return cudaSuccess;
   if (page != kTileTok || (q_ld_t % 8) != 0) return cudaErrorInvalidValue;
-  EncodeTiledFn fn = encode_fn();
-  if (fn == nullptr) return cudaErrorUnknown;
+  // q: [B tokens][16 heads][576] bf16, head stride 576, token stride q_ld_t -> boxes of [1][16][64]
+  TmapSpec sq;
+  sq.ptr = q; sq.rank = 3; sq.l2 = CU_TENSOR_MAP_L2_PROMOTION_L2_128B;
+  sq.dims[0] = kDk; sq.dims[1] = kHeads; sq.dims[2] = B;
+  sq.strides[0] = (uint64_t)kDk * 2; sq.strides[1] = (uint64_t)q_ld_t * 2;
+  sq.box[0] = 64; sq.box[1] = kHeads; sq.box[2] = 1;
+  // latent pool: [num_pages * page][576] bf16 -> boxes of [64 tokens][64]
+  TmapSpec skv;
+  skv.ptr = pool;
+  skv.dims[0] = kDk; skv.dims[1] = (uint64_t)num_pages * page;
+  skv.strides[0] = (uint64_t)kDk * 2;
+  skv.box[0] = 64; skv.box[1] = kTileTok;
   CUtensorMap tq, tkv;
-  {
-    // q: [B tokens][16 heads][576] bf16, head stride 576, token stride q_ld_t -> boxes of [1][16][64]
-    cuuint64_t dims[3] = {(cuuint64_t)kDk, (cuuint64_t)kHeads, (cuuint64_t)B};
-    cuuint64_t strides[2] = {(cuuint64_t)kDk * 2, (cuuint64_t)q_ld_t * 2};
-    cuuint32_t box[3] = {64, (cuuint32_t)kHeads, 1};
-    cuuint32_t estr[3] = {1, 1, 1};
-    if (fn(&tq, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(q), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-           CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-      return cudaErrorInvalidValue;
-  }
-  {
-    cuuint64_t dims[2] = {(cuuint64_t)kDk, (cuuint64_t)num_pages * page};
-    cuuint64_t strides[1] = {(cuuint64_t)kDk * 2};
-    cuuint32_t box[2] = {64, (cuuint32_t)kTileTok};
-    cuuint32_t estr[2] = {1, 1};
-    if (fn(&tkv, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(pool), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-           CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
-      return cudaErrorInvalidValue;
-  }
+  if (!tmap_encode(&tq, sq) || !tmap_encode(&tkv, skv)) return cudaErrorInvalidValue;
   MlaParams p;
   p.block_tables = block_tables; p.max_blocks = max_blocks; p.context_lens = context_lens;
   const int max_tiles = (max_ctx + kTileTok - 1) / kTileTok;
@@ -435,14 +412,10 @@ cudaError_t mla_decode_launch(const void* q, long long q_ld_t, int B, const void
   if (nsplit > 1 && workspace == nullptr) return cudaErrorInvalidValue;
   constexpr int smem = 2 * kTileBytes + kQBytes + 2 * kPBytes + 2 * 4 * kHeads * 4 + 5 * 8 + 1024;
   static_assert(smem <= 227 * 1024, "shared memory budget exceeded");
-  static bool configured = false;
-  if (!configured) {
-    cudaError_t e = cudaFuncSetAttribute(mla_decode_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) return e;
-    configured = true;
-  }
+  cudaError_t e = set_max_dynamic_smem_once<mla_decode_kernel>(smem);
+  if (e != cudaSuccess) return e;
   (void)launch_pdl(mla_decode_kernel, dim3(nsplit, B), dim3(kThreads), smem, s, tq, tkv, p);
-  cudaError_t e = cudaGetLastError();
+  e = cudaGetLastError();
   if (e != cudaSuccess || nsplit == 1) return e;
   (void)launch_pdl(mla_combine_kernel, dim3(B, kHeads), dim3(128), 0, s, (const float*)p.part_o, (const float*)p.part_ml, nsplit,
                    static_cast<__nv_bfloat16*>(out), o_ld_t);

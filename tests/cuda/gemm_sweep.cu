@@ -25,8 +25,9 @@ int main() {
     {"o_proj m256 256x2048x2048", 256, 2048, 2048, false, true},
   };
   cudaStream_t st; CK(cudaStreamCreate(&st));
+  constexpr size_t kWsFloats = 64u << 20;   // 256 MB
   float* ws; unsigned int* ctr;
-  CK(cudaMalloc(&ws, 256u << 20)); CK(cudaMalloc(&ctr, 65536 * 4)); CK(cudaMemset(ctr, 0, 65536 * 4));
+  CK(cudaMalloc(&ws, kWsFloats * 4)); CK(cudaMalloc(&ctr, 65536 * 4)); CK(cudaMemset(ctr, 0, 65536 * 4));
   for (auto& s : shapes) {
     const size_t wbytes = (size_t)s.n * s.k * 2 * (s.dual ? 2 : 1);
     int nrot = (int)((300ull << 20) / wbytes) + 1; if (nrot > 64) nrot = 64;
@@ -41,8 +42,10 @@ int main() {
       if ((s.k / 64) / splits < 2) continue;
       GemmArgs a; a.x = x; a.x_rows = s.m; a.ld_x = s.k; a.ld_w = s.k; a.m = s.m; a.n = s.n; a.k = s.k; a.max_rows = s.m;
       a.out = out; a.ld_out = s.n; if (s.res) { a.residual = res; a.ld_res = s.n; } a.act = kActSilu; a.splits = splits;
-      a.workspace = ws; a.tile_counters = ctr;
-      auto launch = [&](int i) { a.w = w[i % nrot]; a.w2 = s.dual ? w2[i % nrot] : nullptr; cudaError_t e = gemm_launch(a, st); if (e != cudaSuccess) { printf("launch err %s\n", cudaGetErrorString(e)); exit(3); } };
+      a.workspace = ws; a.tile_counters = ctr; a.w2 = s.dual ? w2[0] : nullptr;
+      const GemmPlan plan = gemm_plan(a, kGemmBf16, sm_count());
+      if (plan.workspace_floats > kWsFloats) { printf("workspace of %zu floats does not fit\n", plan.workspace_floats); exit(3); }
+      auto launch = [&](int i) { a.w = w[i % nrot]; a.w2 = s.dual ? w2[i % nrot] : nullptr; cudaError_t e = gemm_launch(a, plan, st); if (e != cudaSuccess) { printf("launch err %s\n", cudaGetErrorString(e)); exit(3); } };
       for (int i = 0; i < nrot; ++i) launch(i);   // warm: descriptors cached, attributes set
       CK(cudaStreamSynchronize(st));
       const int iters = 2 * nrot;

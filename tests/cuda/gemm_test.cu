@@ -51,7 +51,7 @@ __global__ void ref_gemm(const __nv_bfloat16* x, long long ldx, const __nv_bfloa
 
 struct Case {
   std::string name; int m, n, k; bool dual = false, res = false, bias = false, fp32 = false; int splits = 1;
-  int E = 0; int bn = 0; float softcap = 0.f; int act = kActSilu; int ldx_pad = 0; int iters = 0;
+  int E = 0; float softcap = 0.f; int act = kActSilu; int ldx_pad = 0; int iters = 0;
 };
 
 static int run_case(const Case& c) {
@@ -88,15 +88,15 @@ static int run_case(const Case& c) {
   a.x = x; a.x_rows = total_rows; a.ld_x = ldx; a.w = w; a.w2 = w2; a.ld_w = c.k;
   a.m = c.m; a.n = c.n; a.k = c.k; a.max_rows = max_rows; a.num_experts = c.E; a.expert_offsets = d_offs;
   a.out = out; a.ld_out = c.n; a.out_fp32 = c.fp32; a.residual = res; a.ld_res = c.n; a.bias = bias;
-  a.act = c.act; a.softcap = c.softcap; a.bn = c.bn; a.splits = c.splits;
-  int bn = c.bn > 0 ? c.bn : gemm_pick_bn(max_rows);
+  a.act = c.act; a.softcap = c.softcap; a.splits = c.splits;
+  const GemmPlan plan = gemm_plan(a, kGemmBf16, sm_count());
+  const int bn = plan.bn;
   float* ws = nullptr; unsigned int* ctr = nullptr;
-  if (c.splits > 1) {
-    size_t nf = gemm_workspace_floats(a, bn, c.splits);
-    CK(cudaMalloc(&ws, nf * 4)); CK(cudaMalloc(&ctr, 65536 * 4)); CK(cudaMemset(ctr, 0, 65536 * 4));
+  if (plan.workspace_floats > 0) {
+    CK(cudaMalloc(&ws, plan.workspace_floats * 4)); CK(cudaMalloc(&ctr, 65536 * 4)); CK(cudaMemset(ctr, 0, 65536 * 4));
     a.workspace = ws; a.tile_counters = ctr;
   }
-  cudaError_t le = gemm_launch(a, 0);
+  cudaError_t le = gemm_launch(a, plan, 0);
   if (le != cudaSuccess) { printf("[%s] launch failed: %s\n", c.name.c_str(), cudaGetErrorString(le)); return 1; }
   cudaError_t se = cudaDeviceSynchronize();
   if (se != cudaSuccess) { printf("[%s] kernel failed: %s\n", c.name.c_str(), cudaGetErrorString(se)); exit(3); }
@@ -123,16 +123,16 @@ static int run_case(const Case& c) {
   double us = 0;
   if (!fail && c.iters > 0) {
     cudaEvent_t e0, e1; cudaEventCreate(&e0); cudaEventCreate(&e1);
-    for (int i = 0; i < 3; ++i) gemm_launch(a, 0);
+    for (int i = 0; i < 3; ++i) gemm_launch(a, plan, 0);
     cudaEventRecord(e0);
-    for (int i = 0; i < c.iters; ++i) gemm_launch(a, 0);
+    for (int i = 0; i < c.iters; ++i) gemm_launch(a, plan, 0);
     cudaEventRecord(e1); CK(cudaEventSynchronize(e1));
     float ms; cudaEventElapsedTime(&ms, e0, e1); us = ms * 1000.0 / c.iters;
   }
   double wbytes = (double)E * c.n * c.k * 2 * (c.dual ? 2 : 1);
   double flops = 2.0 * total_rows * c.n * (double)c.k * (c.dual ? 2 : 1);
   printf("[%-28s] rows=%d n=%d k=%d bn=%d splits=%d %s max_err=%.4g (max_ref %.3g) bad=%zu nan=%zu", c.name.c_str(), total_rows,
-         c.n, c.k, bn, c.splits, fail ? "FAIL" : "ok", max_err, max_ref, bad, nan);
+         c.n, c.k, bn, plan.splits, fail ? "FAIL" : "ok", max_err, max_ref, bad, nan);
   if (us > 0) printf("  %.1f us  %.0f GB/s(w)  %.1f TFLOP/s", us, wbytes / us * 1e-3, flops / us * 1e-6);
   printf("\n");
   cudaFree(x); cudaFree(w); if (w2) cudaFree(w2); if (res) cudaFree(res); if (bias) cudaFree(bias);
