@@ -22,7 +22,7 @@ OBJ = os.path.join(HERE, "_build")
 MODULE = "_b200_C"
 SO_PATH = os.path.join(HERE, MODULE + ".so")
 
-CU_SOURCES = ["gemm_host.cu", "gemm_tcgen05.cu", "gemm_persistent.cu", "gemm_q_tcgen05.cu", "gemm_q_persistent.cu", "gemm_fp8.cu", "elementwise.cu", "attention.cu", "attention_prefill.cu", "mla_decode.cu", "moe.cu", "sampler.cu", "p2p.cu", "ep.cu"]
+CU_SOURCES = ["gemm_host.cu", "gemm_splitk.cu", "gemm_persistent.cu", "gemm_q_splitk.cu", "gemm_q_persistent.cu", "gemm_fp8.cu", "elementwise.cu", "attention.cu", "attention_prefill.cu", "mla_decode.cu", "moe.cu", "sampler.cu", "p2p.cu", "ep.cu"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ARCH + ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "--use_fast_math",
                      "-Xptxas", "-v"]

@@ -8,7 +8,7 @@
 #include <string>
 #include <vector>
 
-#include "gemm_tcgen05.h"
+#include "gemm.h"
 #include "kernels.h"
 
 namespace py = pybind11;

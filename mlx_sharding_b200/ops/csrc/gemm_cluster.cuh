@@ -37,17 +37,16 @@ B200_DEVICE float ld_dsmem_f32(uint32_t addr) {
 
 // Phase B (MMA warpgroup): reduce this CTA's slice of token columns over the cluster, epilogue, store.
 template <int BN, bool DUAL, typename OutT>
-__device__ __forceinline__ void cluster_epilogue_reduce_store(const GemmParams& p, uint8_t* smem, int epi_base, int n0, int row_base,
-                                                              int rows_valid) {
+__device__ __forceinline__ void cluster_epilogue_reduce_store(const GemmParams& p, uint8_t* smem, const TileInfo& ti) {
   const int S = p.splits;
   const int r = static_cast<int>(cluster_ctarank());
-  const int f_local = threadIdx.x - epi_base;  // 0..127: one feature per thread -> 256 B coalesced rows
-  const int f_glob = n0 + f_local;
+  const int f_local = threadIdx.x;  // 0..127: one feature per thread -> 256 B coalesced rows
+  const int f_glob = ti.n0 + f_local;
   const int per = (BN + S - 1) / S;
   const int t0 = r * per;
   int t1 = t0 + per;
-  if (t1 > rows_valid) t1 = rows_valid;
-  const float bias = (p.bias != nullptr && f_glob < p.n) ? __bfloat162float(p.bias[f_glob]) : 0.0f;
+  if (t1 > ti.rows_valid) t1 = ti.rows_valid;
+  const float bias = feature_bias(p, f_glob);
   const uint32_t local = smem_u32(smem);
   uint32_t peer[8];
 #pragma unroll
@@ -69,13 +68,11 @@ __device__ __forceinline__ void cluster_epilogue_reduce_store(const GemmParams& 
         if (DUAL) u += uv[s];
       }
     }
-    float y = g + bias;
-    if (DUAL) y = apply_act(p.act, y) * u;
-    if (p.softcap > 0.f) y = p.softcap * tanhf(y / p.softcap);
+    float y = epi_value<DUAL>(p, g, u, bias);
     if (f_glob < p.n) {
-      const size_t row = static_cast<size_t>(row_base + t);
+      const size_t row = static_cast<size_t>(ti.row_base + t);
       if (sizeof(OutT) == 2) {
-        // match the non-split path: round the GEMM result to bf16 first, then add the residual
+        // as write_rows: round the GEMM result to bf16 first, then add the residual
         float o = __bfloat162float(__float2bfloat16_rn(y));
         if (p.residual != nullptr) o += __bfloat162float(p.residual[row * p.ld_res + f_glob]);
         reinterpret_cast<__nv_bfloat16*>(p.out)[row * p.ld_out + f_glob] = __float2bfloat16_rn(o);
@@ -88,18 +85,12 @@ __device__ __forceinline__ void cluster_epilogue_reduce_store(const GemmParams& 
   if (p.signal_flag != nullptr) __threadfence_system();
 }
 
-// After the final cluster barrier: one thread of cluster rank 0 ticks the grid-wide completion counter.
-__device__ __forceinline__ void cluster_signal(const GemmParams& p, int epi_base) {
+// After the final cluster barrier: one thread of cluster rank 0 reports the tile as stored.
+__device__ __forceinline__ void cluster_signal(const GemmParams& p) {
   if (p.signal_flag == nullptr) return;
-  if (cluster_ctarank() == 0 && threadIdx.x == static_cast<unsigned>(epi_base)) {
+  if (cluster_ctarank() == 0 && threadIdx.x == 0) {
     __threadfence_system();
-    const unsigned int done = atomicAdd(p.done_counter, 1u) + 1u;
-    if (done == p.signal_tiles) {
-      *p.done_counter = 0u;
-      __threadfence_system();
-      if (p.signal_value == 0u) atomicAdd_system(p.signal_flag, 1u);
-      else st_release_sys(p.signal_flag, p.signal_value);
-    }
+    publish_tiles_done(p, 1u);
   }
 }
 

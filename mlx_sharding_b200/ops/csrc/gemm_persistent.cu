@@ -22,65 +22,17 @@ namespace {
 constexpr int kXBoxRows = 16;                             // token rows per TMA box
 constexpr int kXBoxBytes = kXBoxRows * kBlockK * 2;       // 2 KB
 
-__host__ __device__ constexpr int p_stg_rows(int BN) { return BN < 64 ? BN : 64; }
 // Staging row pitch in elements: 16 B of padding per token row.  A fragment store writes 8 consecutive features of 4 token columns
 // (2 apart); unpadded, those columns are a multiple of 512 B apart and hit the same banks (4-way conflict), padded they are 32 B apart.
 __host__ __device__ constexpr int p_stg_ld(int out_bytes) { return kTileM + 16 / out_bytes; }
-__host__ __device__ constexpr int p_staging_bytes(int BN, int out_bytes) { return p_stg_rows(BN) * p_stg_ld(out_bytes) * out_bytes; }
+__host__ __device__ constexpr int p_staging_bytes(int BN, int out_bytes) { return staging_bytes(BN, p_stg_ld(out_bytes), out_bytes); }
 __host__ __device__ constexpr int p_num_stages(int BN, bool dual, int out_bytes) {
   // 227 KB opt-in shared memory less the 1 KB alignment slack, the staging tile and the barriers (at most 8 stages x 2 x 8 B)
   int s = (227 * 1024 - 1024 - p_staging_bytes(BN, out_bytes) - 2 * 8 * 8) / stage_bytes(BN, dual);
   return s > 8 ? 8 : s;
 }
 
-struct TileInfo {
-  int n0, w_row, row_base, rows_valid, mt;
-};
-
-__device__ __forceinline__ TileInfo decode_tile(const GemmParams& p, int t, int tiles_n, int tiles_m, int BN) {
-  TileInfo ti;
-  const int nt = t % tiles_n;
-  const int rest = t / tiles_n;
-  ti.mt = rest % tiles_m;
-  const int expert = rest / tiles_m;
-  ti.n0 = nt * kTileM;
-  ti.row_base = 0;
-  ti.rows_valid = p.m;
-  if (p.expert_offsets != nullptr) {
-    if (p.expert_stride > 0) {   // scatter layout: fixed stride per expert, the array holds row counts (written by atomics: no __ldg)
-      ti.row_base = expert * p.expert_stride;
-      ti.rows_valid = __ldcg(p.expert_offsets + expert);
-    } else {
-      const int lo = __ldg(p.expert_offsets + expert), hi = __ldg(p.expert_offsets + expert + 1);
-      ti.row_base = lo;
-      ti.rows_valid = hi - lo;
-    }
-  }
-  ti.rows_valid -= ti.mt * BN;
-  ti.row_base += ti.mt * BN;
-  if (ti.rows_valid > BN) ti.rows_valid = BN;
-  ti.w_row = expert * p.n + ti.n0;
-  return ti;
-}
-
 }  // namespace
-
-// One thread per CTA, once, after the CTA's last tile (a system fence per *tile* would stall the epilogue on an NVLink round
-// trip each time when `out` is peer memory): reports how many tiles of the grid this CTA covered; the arrival that completes
-// the grid raises the consumer flag(s) with system scope.  Every CTA fences its own stores before arriving.
-__device__ __forceinline__ void publish_tiles_done(const GemmParams& p, unsigned int n) {
-  const unsigned int done = atomicAdd(p.done_counter, n) + n;
-  if (done != p.signal_tiles) return;
-  *p.done_counter = 0u;
-  __threadfence_system();
-  if (p.signal_peers != nullptr) {
-    for (int i = 0; i < p.num_signal_peers; ++i) atomicAdd_system(reinterpret_cast<unsigned int*>(__ldg(p.signal_peers + i)), 1u);
-  } else if (p.signal_value == 0u) {
-    atomicAdd_system(p.signal_flag, 1u);
-  } else {
-    st_release_sys(p.signal_flag, p.signal_value);
-  }
-}
 
 template <int BN, bool DUAL, typename OutT>
 __global__ void __launch_bounds__(kNumThreads, 1)
@@ -90,7 +42,7 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_
   GemmParams p = p_in;
   constexpr int STAGES = p_num_stages(BN, DUAL, sizeof(OutT));
   constexpr int STAGE_BYTES = stage_bytes(BN, DUAL);
-  constexpr int STG_ROWS = p_stg_rows(BN);
+  constexpr int STG_ROWS = stg_rows(BN);
   constexpr int STG_LD = p_stg_ld(sizeof(OutT));
   constexpr int OFF_X = kATileBytes * (DUAL ? 2 : 1);   // token tile within a stage
   static_assert(STAGES >= 2, "ring too small");
@@ -217,7 +169,6 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_
   } else {
     // ============================================================== MMA warpgroup, then epilogue (128 threads)
     const int et = threadIdx.x;
-    constexpr int kVec = 8, kChunks = kTileM / kVec, kRowsPerIter = kEpiThreads / kChunks;
     uint32_t it = 0, tc = 0, my_tiles = 0;
     bool waited = pdl_early;
     for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
@@ -241,10 +192,7 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_
 #pragma unroll
       for (int h = 0; h < 2; ++h)
 #pragma unroll
-        for (int r = 0; r < 2; ++r) {
-          const int f_glob = ti.n0 + h * 64 + wg_row(2 * r);
-          bias[h][r] = (p.bias != nullptr && f_glob < p.n) ? __bfloat162float(p.bias[f_glob]) : 0.0f;
-        }
+        for (int r = 0; r < 2; ++r) bias[h][r] = feature_bias(p, ti.n0 + h * 64 + wg_row(2 * r));
       // Epilogue on the fragments: acc[h][j] and acc2[h][j] are the same (feature, token).  The chunk loop is unrolled so that the
       // fragment index stays a compile-time constant (the accumulators never leave registers); only valid token columns are stored.
 #pragma unroll
@@ -255,53 +203,11 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_
           const int c = wg_col(j);
           if (c >= ti.rows_valid) continue;
 #pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            float y = acc[h][j] + bias[h][(j >> 1) & 1];
-            if (DUAL) y = apply_act(p.act, y) * acc2[h][j];
-            if (p.softcap > 0.f) y = p.softcap * tanhf(y / p.softcap);
-            stage_store<OutT>(&stg[(c - c0) * STG_LD + h * 64 + wg_row(j)], y);
-          }
+          for (int h = 0; h < 2; ++h)
+            stage_store<OutT>(&stg[(c - c0) * STG_LD + h * 64 + wg_row(j)], epi_value<DUAL>(p, acc[h][j], acc2[h][j], bias[h][(j >> 1) & 1]));
         }
         named_bar_sync(1, kEpiThreads);
-        const int ch = et % kChunks;
-        const int f0 = ti.n0 + ch * kVec;
-        const int rows_here = min(STG_ROWS, ti.rows_valid - c0);
-        if (f0 < p.n) {
-          for (int r = et / kChunks; r < rows_here; r += kRowsPerIter) {
-            const size_t row = static_cast<size_t>(ti.row_base + c0 + r);
-            float vals[kVec];
-            if (sizeof(OutT) == 2) {
-              const uint4 raw = *reinterpret_cast<const uint4*>(reinterpret_cast<const __nv_bfloat16*>(stg) + r * STG_LD + ch * kVec);
-              const uint32_t w4[4] = {raw.x, raw.y, raw.z, raw.w};
-#pragma unroll
-              for (int j = 0; j < 4; ++j) { vals[2 * j] = bf16_lo(w4[j]); vals[2 * j + 1] = bf16_hi(w4[j]); }
-            } else {
-              const float4 a = *reinterpret_cast<const float4*>(reinterpret_cast<const float*>(stg) + r * STG_LD + ch * kVec);
-              const float4 b = *reinterpret_cast<const float4*>(reinterpret_cast<const float*>(stg) + r * STG_LD + ch * kVec + 4);
-              vals[0] = a.x; vals[1] = a.y; vals[2] = a.z; vals[3] = a.w;
-              vals[4] = b.x; vals[5] = b.y; vals[6] = b.z; vals[7] = b.w;
-            }
-            if (p.residual != nullptr) {
-              const uint4 rr = *reinterpret_cast<const uint4*>(p.residual + row * p.ld_res + f0);
-              const uint32_t w4[4] = {rr.x, rr.y, rr.z, rr.w};
-#pragma unroll
-              for (int j = 0; j < 4; ++j) { vals[2 * j] += bf16_lo(w4[j]); vals[2 * j + 1] += bf16_hi(w4[j]); }
-            }
-            // destination row: [row] of `out`, or (EP return) wherever the row's owner wants it — possibly peer memory
-            OutT* orow = p.row_dst != nullptr ? reinterpret_cast<OutT*>(__ldg(p.row_dst + row))
-                                              : reinterpret_cast<OutT*>(p.out) + row * p.ld_out;
-            if (sizeof(OutT) == 2) {
-              uint4 o;
-              o.x = pack_bf16(vals[0], vals[1]); o.y = pack_bf16(vals[2], vals[3]);
-              o.z = pack_bf16(vals[4], vals[5]); o.w = pack_bf16(vals[6], vals[7]);
-              *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(orow) + f0) = o;
-            } else {
-              float* o = reinterpret_cast<float*>(orow) + f0;
-              *reinterpret_cast<float4*>(o) = make_float4(vals[0], vals[1], vals[2], vals[3]);
-              *reinterpret_cast<float4*>(o + 4) = make_float4(vals[4], vals[5], vals[6], vals[7]);
-            }
-          }
-        }
+        write_rows<OutT>(p, stg, STG_LD, et, ti.n0, ti.row_base + c0, min(STG_ROWS, ti.rows_valid - c0));
         named_bar_sync(1, kEpiThreads);  // staging buffer free again
       }
       ++my_tiles;

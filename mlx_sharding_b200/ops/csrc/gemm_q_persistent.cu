@@ -28,33 +28,11 @@ __host__ __device__ constexpr int qp_stage_bytes(int BN, bool dual, int bits) {
   return (BN * kBlockK * 2 + (qp_packed_bytes(bits) + 512) * d + 1023) / 1024 * 1024;
 }
 __host__ __device__ constexpr int qp_dq(int BN, bool dual) { return BN <= 64 && !dual ? 3 : 2; }  // bf16 A-tile buffers
-__host__ __device__ constexpr int qp_stg_rows(int BN) { return BN < 64 ? BN : 64; }
-__host__ __device__ constexpr int qp_staging_bytes(int BN, int out_bytes) { return qp_stg_rows(BN) * kTileM * out_bytes; }
+__host__ __device__ constexpr int qp_staging_bytes(int BN, int out_bytes) { return staging_bytes(BN, kTileM, out_bytes); }
 __host__ __device__ constexpr int qp_num_stages(int BN, bool dual, int bits, int out_bytes) {
   const int fixed = qp_dq(BN, dual) * kATileBytes * (dual ? 2 : 1) + acc_bytes(BN, dual) + qp_staging_bytes(BN, out_bytes) + 1024;
   int s = (225 * 1024 - fixed) / qp_stage_bytes(BN, dual, bits);
   return s > 10 ? 10 : s;
-}
-
-struct QTile { int n0, w_row, row_base, rows_valid; };
-
-__device__ __forceinline__ QTile q_decode_tile(const GemmParams& p, int t, int tiles_n, int tiles_m, int BN) {
-  QTile ti;
-  const int nt = t % tiles_n, rest = t / tiles_n;
-  const int mt = rest % tiles_m, expert = rest / tiles_m;
-  ti.n0 = nt * kTileM;
-  ti.row_base = 0;
-  ti.rows_valid = p.m;
-  if (p.expert_offsets != nullptr) {
-    const int lo = __ldg(p.expert_offsets + expert), hi = __ldg(p.expert_offsets + expert + 1);
-    ti.row_base = lo;
-    ti.rows_valid = hi - lo;
-  }
-  ti.rows_valid -= mt * BN;
-  ti.row_base += mt * BN;
-  if (ti.rows_valid > BN) ti.rows_valid = BN;
-  ti.w_row = expert * p.n + ti.n0;
-  return ti;
 }
 
 }  // namespace
@@ -74,7 +52,6 @@ gemm_q_persistent_kernel(const __grid_constant__ CUtensorMap tmap_wq, const __gr
   constexpr int OFF_SCALE = OFF_PACKED + PACKED_BYTES * D;
   constexpr uint32_t TX_BYTES = BN * kBlockK * 2 + (PACKED_BYTES + 512) * D;
   constexpr int DQ = qp_dq(BN, DUAL);
-  constexpr int STG_ROWS = qp_stg_rows(BN);
   static_assert(STAGES >= 2, "ring too small");
 
   extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -121,7 +98,7 @@ gemm_q_persistent_kernel(const __grid_constant__ CUtensorMap tmap_wq, const __gr
     if (elect_one()) {  // one elected lane: uniform-datapath issue, no per-instruction ELECT loop (ptx.cuh)
       uint32_t it = 0;
       for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-        const QTile ti = q_decode_tile(p, t, tiles_n, tiles_m, BN);
+        const TileInfo ti = decode_tile(p, t, tiles_n, tiles_m, BN);
         if (ti.rows_valid <= 0) continue;
         for (int kb = 0; kb < kb_total; ++kb, ++it) {
           const uint32_t s = it % STAGES, ph = (it / STAGES) & 1;
@@ -143,13 +120,10 @@ gemm_q_persistent_kernel(const __grid_constant__ CUtensorMap tmap_wq, const __gr
     }
   } else if (warp < 4) {
     // ============================================================== MMA warpgroup, then epilogue (128 threads)
-    const int f_local = threadIdx.x;
-    const int et = threadIdx.x;
     const bool leader = lane == 0;
-    constexpr int kVec = 8, kChunks = kTileM / kVec, kRowsPerIter = kEpiThreads / kChunks;
-    uint32_t it = 0;
+    uint32_t it = 0, tc = 0;
     for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-      const QTile ti = q_decode_tile(p, t, tiles_n, tiles_m, BN);
+      const TileInfo ti = decode_tile(p, t, tiles_n, tiles_m, BN);
       if (ti.rows_valid <= 0) continue;
       float acc[2][BN / 2], acc2[2][BN / 2];
       acc_zero<BN>(acc);
@@ -184,87 +158,21 @@ gemm_q_persistent_kernel(const __grid_constant__ CUtensorMap tmap_wq, const __gr
       acc_store_smem<BN>(acc, acc_smem, 0);
       if (DUAL) acc_store_smem<BN>(acc2, acc_smem, BN);
       named_bar_sync(1, kEpiThreads);
-      const int f_glob = ti.n0 + f_local;
-      const float bias = (p.bias != nullptr && f_glob < p.n) ? __bfloat162float(p.bias[f_glob]) : 0.0f;
-#pragma unroll 1
-      for (int c0 = 0; c0 < BN; c0 += STG_ROWS) {
-        if (c0 >= ti.rows_valid) break;
-#pragma unroll 1
-        for (int c = c0; c < c0 + STG_ROWS; c += 16) {
-          if (c >= ti.rows_valid) break;
-          float g[16], u[16];
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            g[j] = acc_smem[(c + j) * kTileM + f_local];
-            if (DUAL) u[j] = acc_smem[(BN + c + j) * kTileM + f_local];
-          }
-#pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            float y = g[j] + bias;
-            if (DUAL) y = apply_act(p.act, y) * u[j];
-            if (p.softcap > 0.f) y = p.softcap * tanhf(y / p.softcap);
-            stage_store<OutT>(&stg[(c - c0 + j) * kTileM + f_local], y);
-          }
-        }
-        named_bar_sync(1, kEpiThreads);
-        const int ch = et % kChunks;
-        const int f0 = ti.n0 + ch * kVec;
-        const int rows_here = min(STG_ROWS, ti.rows_valid - c0);
-        if (f0 < p.n) {
-          for (int r = et / kChunks; r < rows_here; r += kRowsPerIter) {
-            const size_t row = static_cast<size_t>(ti.row_base + c0 + r);
-            float vals[kVec];
-            if (sizeof(OutT) == 2) {
-              const uint4 raw = *reinterpret_cast<const uint4*>(reinterpret_cast<const __nv_bfloat16*>(stg) + r * kTileM + ch * kVec);
-              const uint32_t w4[4] = {raw.x, raw.y, raw.z, raw.w};
-#pragma unroll
-              for (int j = 0; j < 4; ++j) { vals[2 * j] = bf16_lo(w4[j]); vals[2 * j + 1] = bf16_hi(w4[j]); }
-            } else {
-              const float4 a = *reinterpret_cast<const float4*>(reinterpret_cast<const float*>(stg) + r * kTileM + ch * kVec);
-              const float4 b = *reinterpret_cast<const float4*>(reinterpret_cast<const float*>(stg) + r * kTileM + ch * kVec + 4);
-              vals[0] = a.x; vals[1] = a.y; vals[2] = a.z; vals[3] = a.w;
-              vals[4] = b.x; vals[5] = b.y; vals[6] = b.z; vals[7] = b.w;
-            }
-            if (p.residual != nullptr) {
-              const uint4 rr = *reinterpret_cast<const uint4*>(p.residual + row * p.ld_res + f0);
-              const uint32_t w4[4] = {rr.x, rr.y, rr.z, rr.w};
-#pragma unroll
-              for (int j = 0; j < 4; ++j) { vals[2 * j] += bf16_lo(w4[j]); vals[2 * j + 1] += bf16_hi(w4[j]); }
-            }
-            if (sizeof(OutT) == 2) {
-              uint4 o;
-              o.x = pack_bf16(vals[0], vals[1]); o.y = pack_bf16(vals[2], vals[3]);
-              o.z = pack_bf16(vals[4], vals[5]); o.w = pack_bf16(vals[6], vals[7]);
-              *reinterpret_cast<uint4*>(reinterpret_cast<__nv_bfloat16*>(p.out) + row * p.ld_out + f0) = o;
-            } else {
-              float* o = reinterpret_cast<float*>(p.out) + row * p.ld_out + f0;
-              *reinterpret_cast<float4*>(o) = make_float4(vals[0], vals[1], vals[2], vals[3]);
-              *reinterpret_cast<float4*>(o + 4) = make_float4(vals[4], vals[5], vals[6], vals[7]);
-            }
-          }
-        }
-        named_bar_sync(1, kEpiThreads);
-      }
-      if (p.signal_flag != nullptr) {
-        __threadfence_system();
-        named_bar_sync(1, kEpiThreads);
-        if (et == 0) {
-          const unsigned int done = atomicAdd(p.done_counter, 1u) + 1u;
-          if (done == p.signal_tiles) {
-            *p.done_counter = 0u;
-            __threadfence_system();
-            if (p.signal_value == 0u) atomicAdd_system(p.signal_flag, 1u);
-            else st_release_sys(p.signal_flag, p.signal_value);
-          }
-        }
-      }
+      store_acc_tile<BN, DUAL, OutT>(p, acc_smem, stg, ti);
+      ++tc;
+    }
+    if (p.signal_flag != nullptr) {
+      // fused stage boundary: fence once, then report this CTA's tiles
+      __threadfence_system();
+      named_bar_sync(1, kEpiThreads);
+      if (threadIdx.x == 0) publish_tiles_done(p, tc);
     }
   } else {
     // ============================================================== dequant producers (4 warps, one thread per row)
     const int r = threadIdx.x - kNumThreads;
     uint32_t it = 0;
     for (int t = blockIdx.x; t < num_tiles; t += gridDim.x) {
-      const QTile ti = q_decode_tile(p, t, tiles_n, tiles_m, BN);
+      const TileInfo ti = decode_tile(p, t, tiles_n, tiles_m, BN);
       if (ti.rows_valid <= 0) continue;
       for (int kb = 0; kb < kb_total; ++kb, ++it) {
         const uint32_t s = it % STAGES, ph = (it / STAGES) & 1;

@@ -9,7 +9,7 @@ stage ``i+1``'s inbox, and the last stage one into stage 0's token inbox.
 Hand-off = the *last kernel of the stage* (the down-proj wgmma GEMM epilogue for dense layers, the
 MoE weighted-combine for DeepSeek MoE layers) stores its output rows straight into the peer inbox and
 the last CTA bumps the peer's flag with a system-scope release (``models/base.py::_final_kwargs``,
-``csrc/gemm_tcgen05.cu``, ``csrc/moe.cu``).  The consumer's step begins with a one-thread
+``csrc/gemm_splitk.cu``, ``csrc/moe.cu``).  The consumer's step begins with a one-thread
 ``wait_flag_counter`` kernel (acquire.sys spin, bounded) — so a decode step is a single CUDA-graph
 launch per stage with **no NCCL call, no host hop and no host->device traffic**.  Compare with the
 reference: one blocking gRPC unary call per stage per token, host-staged fp16 (shard/utils.py:71-90,162-164).

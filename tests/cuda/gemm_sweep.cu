@@ -4,7 +4,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <vector>
-#include "../../mlx_sharding_b200/ops/csrc/gemm_tcgen05.h"
+#include "../../mlx_sharding_b200/ops/csrc/gemm.h"
 using namespace b200;
 #define CK(x) do { cudaError_t e_ = (x); if (e_ != cudaSuccess) { printf("CUDA error %s at %s:%d\n", cudaGetErrorString(e_), __FILE__, __LINE__); exit(2); } } while (0)
 

@@ -5,7 +5,7 @@
 #include <cmath>
 #include <vector>
 #include <string>
-#include "../../mlx_sharding_b200/ops/csrc/gemm_tcgen05.h"
+#include "../../mlx_sharding_b200/ops/csrc/gemm.h"
 
 using namespace b200;
 
