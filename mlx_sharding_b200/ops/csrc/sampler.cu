@@ -26,10 +26,17 @@ __device__ __forceinline__ uint64_t mix64(uint64_t z) {
   z = (z ^ (z >> 27)) * 0x94D049BB133111EBull;
   return z ^ (z >> 31);
 }
+// u = (k + 0.5) / 2^23 for the top 23 hash bits k, so 2^-24 <= u <= 1 - 2^-24.  Both u and u - 1 are exact in fp32 (a 24-bit k
+// would round (2^24 - 1) + 0.5 up to 2^24, giving u = 1).
 __device__ __forceinline__ float uniform01(uint64_t seed, uint64_t step, uint32_t row, uint32_t i) {
   const uint64_t h = mix64(mix64(seed ^ (step * 0xD1342543DE82EF95ull)) ^ ((uint64_t)row << 32 | i));
-  return ((float)(h >> 40) + 0.5f) * (1.0f / 16777216.0f);  // (0, 1)
+  return ((float)(uint32_t)(h >> 41) + 0.5f) * (1.0f / 8388608.0f);
 }
+// Gumbel noise g = -log(-log(u)), finite for every u above (-log(u) lies in [6e-8, 16.6], g in [-2.81, 16.6]).  The draw is
+// decided by the ids with u near 1, where -log(u) is tiny: it comes from log1pf of the exact u - 1 at full precision
+// (--use_fast_math compiles logf to __logf, whose absolute error near 1 is as large as -log(u) itself).  The outer __logf adds
+// about 1e-7 absolute error to g.
+__device__ __forceinline__ float gumbel(float u) { return -__logf(-log1pf(u - 1.0f)); }
 
 struct ArgMax { float v; int i; };
 __device__ __forceinline__ ArgMax better(ArgMax a, ArgMax b) {
@@ -168,9 +175,7 @@ __device__ __forceinline__ int draw_token(const float* __restrict__ lg, const ui
   for (int i = threadIdx.x; i < V; i += kSampThreads) {
     const float x = draw_logit<kMask>(lg, al, i);
     if (x > thresh && (!kFilt || x >= floor)) {
-      const float u = uniform01(seed, step, rng_row, i);
-      const float g = -__logf(-__logf(u));
-      gm = better(gm, ArgMax{(x - amv) * inv_t + g, i});
+      gm = better(gm, ArgMax{(x - amv) * inv_t + gumbel(uniform01(seed, step, rng_row, i)), i});
     }
   }
   gm = block_argmax(gm, sm_a);
