@@ -361,8 +361,7 @@ class DeepseekV2Stage(StageModel):
                 self._prenormed = res
                 return res[0]
             return res
-        if ("router" in w and ep is not None and hasattr(ep, "route_forward") and getattr(ep.b, "v2", False)
-                and 1 <= T <= 1024 and os.environ.get("MLXB200_EP_FUSED_ROUTE", "1") != "0"):
+        if "router" in w and hasattr(ep, "route_forward") and 1 <= T <= 1024:
             # expert-parallel block as four kernels (parallel/ep.py::route_forward): [pre-MoE norm + router + dispatch] -> grouped
             # gate/up -> grouped down (+ return) -> [combine + next layer's input norm]; the shared experts fork onto the side
             # stream right behind the router (they consume the normalised rows it stores)

@@ -662,26 +662,27 @@ void advance_meta(Tensor positions, Tensor context_lens, Tensor slots, const Ten
 }
 
 // ---- expert parallel --------------------------------------------------------------------------------------------
-std::vector<unsigned long long> to_u64(const std::vector<int64_t>& v) {
-  std::vector<unsigned long long> o(v.size());
-  for (size_t i = 0; i < v.size(); ++i) o[i] = (unsigned long long)v[i];
-  return o;
-}
-void ep_dispatch(const Tensor& x, const Tensor& idx, int64_t experts_per_rank, int64_t my_rank, int64_t cap,
-                 std::vector<int64_t> recv_x, std::vector<int64_t> recv_meta, std::vector<int64_t> recv_words, Tensor send_seq,
-                 Tensor send_counts, Tensor done_counter, const c10::optional<Tensor>& ret_expected) {
-  check_bf16(x, "x"); check_rows(x, "x");
-  TORCH_CHECK(idx.scalar_type() == torch::kInt32 && idx.is_contiguous() && idx.dim() == 2);
-  const c10::cuda::CUDAGuard guard(x.device());
+// One dispatch step's destinations: peer tables (one address per rank) and this rank's step state, shared by both dispatch launches.
+b200::EpDispatch ep_dispatch_args(int64_t experts_per_rank, int64_t my_rank, int64_t cap_e, const std::vector<int64_t>& recv_x,
+                                  const std::vector<int64_t>& recv_dst, const std::vector<int64_t>& recv_cnt,
+                                  const std::vector<int64_t>& recv_seq, const std::vector<int64_t>& my_ret, Tensor& send_seq,
+                                  Tensor& done_counter, const c10::optional<Tensor>& ret_expected) {
   const int world = (int)recv_x.size();
-  auto a = to_u64(recv_x), b = to_u64(recv_meta), c = to_u64(recv_words);
-  LAUNCH_OK(b200::ep_dispatch_launch(x.data_ptr(), x.stride(0), idx.data_ptr<int>(), (int)idx.numel(), (int)idx.size(1), (int)x.size(1),
-                                     (int)experts_per_rank, world, (int)my_rank, (int)cap, a.data(), b.data(), c.data(),
-                                     reinterpret_cast<uint32_t*>(send_seq.data_ptr<int>()), send_counts.data_ptr<int>(),
-                                     reinterpret_cast<unsigned int*>(done_counter.data_ptr<int>()),
-                                     ret_expected.has_value() ? reinterpret_cast<uint32_t*>(ret_expected->data_ptr<int>()) : nullptr,
-                                     cur_stream()));
+  TORCH_CHECK(world >= 1 && world <= b200::kEpMaxWorld, "expert parallelism supports 1 to ", b200::kEpMaxWorld, " ranks");
+  TORCH_CHECK((int)recv_dst.size() == world && (int)recv_cnt.size() == world && (int)recv_seq.size() == world && (int)my_ret.size() == world,
+              "every peer table needs one address per rank");
+  b200::EpDispatch ep;
+  ep.enabled = 1; ep.experts_per_rank = (int)experts_per_rank; ep.world = world; ep.my_rank = (int)my_rank; ep.cap_e = (int)cap_e;
+  auto fill = [&](b200::EpPeerTable& t, const std::vector<int64_t>& v) {
+    for (int i = 0; i < b200::kEpMaxWorld; ++i) t.p[i] = i < world ? (unsigned long long)v[i] : 0ull;
+  };
+  fill(ep.recv_x, recv_x); fill(ep.recv_dst, recv_dst); fill(ep.recv_cnt, recv_cnt); fill(ep.recv_seq, recv_seq); fill(ep.my_ret, my_ret);
+  ep.send_seq = reinterpret_cast<uint32_t*>(send_seq.data_ptr<int>());
+  ep.done_counter = reinterpret_cast<unsigned int*>(done_counter.data_ptr<int>());
+  ep.ret_expected = ret_expected.has_value() ? reinterpret_cast<uint32_t*>(ret_expected->data_ptr<int>()) : nullptr;
+  return ep;
 }
+
 void ep_dispatch_scatter(const Tensor& x, const Tensor& idx, int64_t experts_per_rank, int64_t my_rank, int64_t cap_e,
                          std::vector<int64_t> recv_x, std::vector<int64_t> recv_dst, std::vector<int64_t> recv_cnt,
                          std::vector<int64_t> recv_seq, std::vector<int64_t> my_ret, Tensor send_seq, Tensor done_counter,
@@ -689,18 +690,14 @@ void ep_dispatch_scatter(const Tensor& x, const Tensor& idx, int64_t experts_per
   check_bf16(x, "x"); check_rows(x, "x");
   TORCH_CHECK(idx.scalar_type() == torch::kInt32 && idx.is_contiguous() && idx.dim() == 2);
   const c10::cuda::CUDAGuard guard(x.device());
-  const int world = (int)recv_x.size();
-  auto a = to_u64(recv_x), b = to_u64(recv_dst), c = to_u64(recv_cnt), d = to_u64(recv_seq), e = to_u64(my_ret);
+  const b200::EpDispatch ep = ep_dispatch_args(experts_per_rank, my_rank, cap_e, recv_x, recv_dst, recv_cnt, recv_seq, my_ret, send_seq,
+                                               done_counter, ret_expected);
   LAUNCH_OK(b200::ep_dispatch_scatter_launch(x.data_ptr(), x.stride(0), idx.data_ptr<int>(), (int)idx.numel(), (int)idx.size(1), (int)x.size(1),
-                                             (int)experts_per_rank, world, (int)my_rank, (int)cap_e, a.data(), b.data(), c.data(), d.data(),
-                                             e.data(), reinterpret_cast<uint32_t*>(send_seq.data_ptr<int>()),
-                                             reinterpret_cast<unsigned int*>(done_counter.data_ptr<int>()),
-                                             ret_expected.has_value() ? reinterpret_cast<uint32_t*>(ret_expected->data_ptr<int>()) : nullptr,
-                                             cur_stream()));
+                                             ep, cur_stream()));
 }
 
-// Router + expert-parallel dispatch in one kernel (v2 exchange): returns {idx, wts}; optionally normalises `x` first (norm_w) and
-// stores the normalised rows (normed_out) for the shared-expert branch.
+// Router + expert-parallel dispatch in one kernel: returns {idx, wts}; optionally normalises `x` first (norm_w) and stores the
+// normalised rows (normed_out) for the shared-expert branch.
 std::vector<Tensor> ep_route_dispatch(const Tensor& x, const Tensor& gate_w, int64_t top_k, int64_t n_group, int64_t topk_group, double scaling,
                                       bool norm_topk, int64_t experts_per_rank, int64_t my_rank, int64_t cap_e, std::vector<int64_t> recv_x,
                                       std::vector<int64_t> recv_dst, std::vector<int64_t> recv_cnt, std::vector<int64_t> recv_seq,
@@ -709,22 +706,14 @@ std::vector<Tensor> ep_route_dispatch(const Tensor& x, const Tensor& gate_w, int
   check_bf16(x, "x"); check_bf16(gate_w, "gate_w"); check_rows(x, "x");
   TORCH_CHECK(gate_w.is_contiguous());
   const c10::cuda::CUDAGuard guard(x.device());
-  const int T = (int)x.size(0), world = (int)recv_x.size();
-  TORCH_CHECK(T >= 1 && T <= 1024 && world <= b200::kEpMaxWorld, "fused route + dispatch needs 1 <= T <= 1024");
+  const int T = (int)x.size(0);
+  TORCH_CHECK(T >= 1 && T <= 1024, "fused route + dispatch needs 1 <= T <= 1024");
   if (norm_w.has_value()) { check_bf16(*norm_w, "norm_w"); TORCH_CHECK(norm_w->is_contiguous() && norm_w->numel() == x.size(1)); }
   if (normed_out.has_value()) { check_bf16(*normed_out, "normed_out"); check_rows(*normed_out, "normed_out"); TORCH_CHECK(normed_out->size(0) >= T && normed_out->size(1) == x.size(1)); }
   Tensor idx = torch::empty({T, top_k}, torch::dtype(torch::kInt32).device(x.device()));
   Tensor w = torch::empty({T, top_k}, torch::dtype(torch::kFloat32).device(x.device()));
-  b200::RouteEP ep;
-  ep.enabled = 1; ep.experts_per_rank = (int)experts_per_rank; ep.world = world; ep.my_rank = (int)my_rank; ep.cap_e = (int)cap_e;
-  auto fill = [&](b200::EpPeerTable& t, const std::vector<int64_t>& v) {
-    for (int i = 0; i < b200::kEpMaxWorld; ++i) t.p[i] = i < world ? (unsigned long long)v[i] : 0ull;
-  };
-  TORCH_CHECK((int)recv_dst.size() == world && (int)recv_cnt.size() == world && (int)recv_seq.size() == world && (int)my_ret.size() == world);
-  fill(ep.recv_x, recv_x); fill(ep.recv_dst, recv_dst); fill(ep.recv_cnt, recv_cnt); fill(ep.recv_seq, recv_seq); fill(ep.my_ret, my_ret);
-  ep.send_seq = reinterpret_cast<uint32_t*>(send_seq.data_ptr<int>());
-  ep.done_counter = reinterpret_cast<unsigned int*>(done_counter.data_ptr<int>());
-  ep.ret_expected = ret_expected.has_value() ? reinterpret_cast<uint32_t*>(ret_expected->data_ptr<int>()) : nullptr;
+  const b200::EpDispatch ep = ep_dispatch_args(experts_per_rank, my_rank, cap_e, recv_x, recv_dst, recv_cnt, recv_seq, my_ret, send_seq,
+                                               done_counter, ret_expected);
   LAUNCH_OK(b200::moe_route_launch(x.data_ptr(), x.stride(0), gate_w.data_ptr(), T, (int)x.size(1), (int)gate_w.size(0), (int)top_k,
                                    (int)n_group, (int)topk_group, (float)scaling, norm_topk, 0, idx.data_ptr<int>(), w.data_ptr<float>(),
                                    nullptr, 0, nullptr, nullptr, norm_w.has_value() ? norm_w->data_ptr() : nullptr, (float)norm_eps,
@@ -733,30 +722,6 @@ std::vector<Tensor> ep_route_dispatch(const Tensor& x, const Tensor& gate_w, int
   return {idx, w};
 }
 
-std::vector<Tensor> ep_regroup(int64_t recv_words_ptr, int64_t counter_ptr, int64_t error_ptr, int64_t recv_meta_ptr,
-                               int64_t recv_x_ptr, int64_t world, int64_t cap, int64_t E_local, int64_t H, int64_t device,
-                               int64_t rows_bound, std::vector<int64_t> ret_y) {
-  auto dev = torch::Device(torch::kCUDA, (int)device);
-  const c10::cuda::CUDAGuard guard(dev);
-  auto io = torch::dtype(torch::kInt32).device(dev);
-  // rows_bound (>0): the caller's bound on the rows all sources can send this step; sizes the expert-ordered temporaries
-  const int64_t R = rows_bound > 0 ? std::min<int64_t>(world * cap, rows_bound) : world * cap;
-  Tensor offs = torch::empty({E_local + 1}, io), row_perm = torch::empty({world * cap}, io), total = torch::empty({1}, io);
-  Tensor counts = torch::empty({world}, io);
-  Tensor x_perm = torch::empty({R, H}, torch::dtype(torch::kBFloat16).device(dev));
-  // destination address of every expert-ordered row for the fused return (down-projection epilogue -> source's return buffer)
-  Tensor row_dst = torch::empty({ret_y.empty() ? 0 : R}, torch::dtype(torch::kInt64).device(dev));
-  auto ry = to_u64(ret_y);
-  LAUNCH_OK(b200::ep_regroup_launch(reinterpret_cast<const unsigned long long*>(recv_words_ptr), reinterpret_cast<uint32_t*>(counter_ptr),
-                                    reinterpret_cast<uint32_t*>(error_ptr), counts.data_ptr<int>(),
-                                    reinterpret_cast<const void*>(recv_meta_ptr), reinterpret_cast<const void*>(recv_x_ptr), (int)world,
-                                    (int)cap, (int)E_local, (int)H, offs.data_ptr<int>(), row_perm.data_ptr<int>(), total.data_ptr<int>(),
-                                    x_perm.data_ptr(), ret_y.empty() ? nullptr : ry.data(),
-                                    ret_y.empty() ? nullptr : reinterpret_cast<unsigned long long*>(row_dst.data_ptr<int64_t>()),
-                                    cur_stream()));
-  ++g_launches;
-  return {offs, total, x_perm, row_dst};
-}
 Tensor ep_combine(int64_t flag_ptr, const Tensor& expected, int64_t error_ptr, const Tensor& ret_y, const Tensor& wts,
                   const c10::optional<Tensor>& residual, const c10::optional<Tensor>& out_, const c10::optional<Tensor>& norm_w,
                   double norm_eps, const c10::optional<Tensor>& normed) {
@@ -838,15 +803,9 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
   m.def("set_flag", &set_flag);
   m.def("copy_signal", &copy_signal);
   m.def("advance_meta", &advance_meta);
-  m.def("ep_dispatch", &ep_dispatch, py::arg("x"), py::arg("idx"), py::arg("experts_per_rank"), py::arg("my_rank"), py::arg("cap"),
-        py::arg("recv_x"), py::arg("recv_meta"), py::arg("recv_words"), py::arg("send_seq"), py::arg("send_counts"),
-        py::arg("done_counter"), py::arg("ret_expected") = py::none());
   m.def("ep_dispatch_scatter", &ep_dispatch_scatter, py::arg("x"), py::arg("idx"), py::arg("experts_per_rank"), py::arg("my_rank"),
         py::arg("cap_e"), py::arg("recv_x"), py::arg("recv_dst"), py::arg("recv_cnt"), py::arg("recv_seq"), py::arg("my_ret"),
         py::arg("send_seq"), py::arg("done_counter"), py::arg("ret_expected") = py::none());
-  m.def("ep_regroup", &ep_regroup, py::arg("recv_words_ptr"), py::arg("counter_ptr"), py::arg("error_ptr"),
-        py::arg("recv_meta_ptr"), py::arg("recv_x_ptr"), py::arg("world"), py::arg("cap"), py::arg("E_local"), py::arg("H"),
-        py::arg("device"), py::arg("rows_bound") = 0, py::arg("ret_y") = std::vector<int64_t>());
   m.def("ep_combine", &ep_combine, py::arg("flag_ptr"), py::arg("expected"), py::arg("error_ptr"), py::arg("ret_y"), py::arg("wts"),
         py::arg("residual") = py::none(), py::arg("out") = py::none(), py::arg("norm_w") = py::none(), py::arg("norm_eps") = 1e-6,
         py::arg("normed") = py::none());

@@ -16,9 +16,11 @@ struct GemmParams {
   // block-scaled FP8 (gemm_fp8.cu): ue8m0 scale words (4 scales = one 128-element k-block per uint32), row-major [rows, K / 128]
   const uint32_t* w_sf; const uint32_t* w2_sf; const uint32_t* x_sf;
   int sf_ld_w, sf_ld_x;
-  // Expert-parallel receive side (ep.cu v2, gemm_persistent.cu only): before touching tokens / counts the kernel waits until every
-  // source rank has published this step's sequence number (ep_arrive[r], acquire.sys); counts are double-buffered by step parity
-  const unsigned long long* ep_arrive; const uint32_t* ep_seq; uint32_t* ep_error; int ep_world; int ep_zero_other;
+  // Expert-parallel receive side (ep.cu, gemm_persistent.cu only): before touching tokens / counts the kernel waits until every
+  // source rank has published this step's sequence number (ep_arrive[r], acquire.sys), for at most ep_timeout_ns (wait_timeout_ns);
+  // counts are double-buffered by step parity
+  const unsigned long long* ep_arrive; const uint32_t* ep_seq; uint32_t* ep_error; unsigned long long ep_timeout_ns;
+  int ep_world; int ep_zero_other;
   int expert_stride;  // > 0: experts live at fixed row stride, expert_offsets[e] is the row COUNT of expert e (scatter layout)
   void* out;
   long long ld_out;

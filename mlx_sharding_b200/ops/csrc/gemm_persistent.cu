@@ -11,6 +11,7 @@
 // 64-row segment.
 #include "gemm_common.cuh"
 #include "gemm_tmap.h"
+#include "kernels.h"
 #include "launch.h"
 
 namespace b200 {
@@ -77,20 +78,13 @@ gemm_persistent_kernel(const __grid_constant__ CUtensorMap tmap_w, const __grid_
   if (p.ep_arrive != nullptr) {
     // Expert-parallel receive side: the token rows, their return addresses and the per-expert row counts of this step are written
     // into this rank's buffers by the *other ranks'* dispatch kernels.  Each source publishes the step's sequence number with
-    // release.sys after its rows; one thread per CTA acquires all of them (bounded spin), then the whole CTA proceeds.  This wait
-    // used to be a separate single-CTA kernel followed by a gather; now the persistent GEMM's CTAs are already resident (PDL).
+    // release.sys after its rows (ep_dispatch.cuh); one thread per CTA acquires all of them, then the whole CTA proceeds.
     if (threadIdx.x == 0) {
       const uint32_t expected = *reinterpret_cast<const volatile uint32_t*>(p.ep_seq);   // == my own dispatch count (lock-step ranks)
-      unsigned long long t0;
-      asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t0));
-      for (int r = 0; r < p.ep_world; ++r) {
-        while (static_cast<uint32_t>(ld_acquire_sys_u64(p.ep_arrive + r)) != expected) {
-          unsigned long long t1;
-          asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t1));
-          if (t1 - t0 > 20000000000ull) { if (p.ep_error != nullptr) atomicExch(p.ep_error, 1u); break; }
-          __nanosleep(32);
-        }
-      }
+      const unsigned long long t0 = globaltimer_ns();
+      for (int r = 0; r < p.ep_world; ++r)
+        spin_acquire([&] { return static_cast<uint32_t>(ld_acquire_sys_u64(p.ep_arrive + r)) == expected; }, t0, p.ep_timeout_ns,
+                     p.ep_error);
       __threadfence_system();
     }
     __syncthreads();
@@ -249,7 +243,10 @@ cudaError_t gemm_persistent_launch(const GemmArgs& a, const GemmPlan& plan, cuda
   GemmMaps t;
   if (!gemm_maps(a, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, kXBoxRows, &t)) return cudaErrorUnknown;
   GemmParams p = gemm_params(a, plan);
-  p.ep_arrive = a.ep_arrive; p.ep_seq = a.ep_seq; p.ep_error = a.ep_error; p.ep_world = a.ep_world; p.ep_zero_other = a.ep_zero_other ? 1 : 0;
+  if (a.ep_arrive != nullptr) {
+    p.ep_arrive = a.ep_arrive; p.ep_seq = a.ep_seq; p.ep_error = a.ep_error; p.ep_timeout_ns = wait_timeout_ns();
+    p.ep_world = a.ep_world; p.ep_zero_other = a.ep_zero_other ? 1 : 0;
+  }
   if (a.signal_peers != nullptr) {
     // EP return: every tile of the grid (empty experts included) is counted, then all peers are signalled
     p.row_dst = a.row_dst; p.signal_peers = a.signal_peers; p.num_signal_peers = a.num_signal_peers;

@@ -4,6 +4,8 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include <cstdlib>
+
 namespace b200 {
 
 // ---- elementwise.cu
@@ -66,15 +68,15 @@ cudaError_t mla_decode_launch(const void* q, long long q_ld_t, int B, const void
                               const int* block_tables, int max_blocks, const int* context_lens, int max_ctx, float scale,
                               int nsplit, float* workspace, void* out, long long o_ld_t, long long* dbg, cudaStream_t s);
 
-// ---- expert-parallel peer tables (ep.cu, and the router's fused dispatch in moe.cu)
+// ---- expert-parallel dispatch (ep.cu, and the router's fused dispatch in moe.cu; device side in ep_dispatch.cuh)
 constexpr int kEpMaxWorld = 16;
 struct EpPeerTable {
   unsigned long long p[kEpMaxWorld];
 };
-// Fused router + expert-parallel dispatch (v2 exchange, see ep.cu): the router CTA of a token reserves the slots of its top-k pairs
-// in the owners' expert-major receive buffers (remote atomics), stores the (normalised) row there and takes part in the
-// publication protocol of ep_dispatch_scatter_kernel — one kernel instead of norm + route + dispatch.
-struct RouteEP {
+// Where one rank's dispatch step writes: per destination rank, its expert-major receive rows, their return addresses, the
+// parity-double-buffered per-expert row counters, the arrival words, and this rank's return buffer as that destination maps it.
+// The router (moe_route_launch with `enabled`) and ep_dispatch_scatter_launch take the same description.
+struct EpDispatch {
   int enabled = 0, experts_per_rank = 0, world = 0, my_rank = 0, cap_e = 0;
   EpPeerTable recv_x, recv_dst, recv_cnt, recv_seq, my_ret;
   uint32_t* send_seq = nullptr;
@@ -88,7 +90,7 @@ struct RouteEP {
 cudaError_t moe_route_launch(const void* x, long long ld_x, const void* gate_w, int T, int H, int E, int top_k,
                              int n_group, int topk_group, float scaling, bool norm_topk, int extra, int* idx, float* wts,
                              int* sc_counts, int sc_stride, int* sc_pair_row, void* sc_x, const void* norm_w, float norm_eps,
-                             cudaStream_t s, const RouteEP* ep = nullptr, void* normed_out = nullptr, long long ld_normed = 0);
+                             cudaStream_t s, const EpDispatch* ep = nullptr, void* normed_out = nullptr, long long ld_normed = 0);
 // (normed_out: also store the normalised row — the shared-expert branch of an expert-parallel block consumes it)
 // (norm_w != nullptr: `x` is the un-normalised residual stream; the router normalises the row in shared memory first — the fused
 //  pre-MoE RMSNorm — so logits and scattered expert inputs equal what a separate norm kernel would have produced)
@@ -121,6 +123,17 @@ cudaError_t sample_launch(const float* logits, int B, int V, const float* temper
                           float* top_lp, const void* tag_src, void* tag_dst, cudaStream_t s);
 
 // ---- p2p.cu
+// Bound of every device-side flag wait (stage hand-off, expert-exchange arrivals and returns): MLXB200_P2P_TIMEOUT_S seconds,
+// default 20.  A wait that runs out sets its error word and returns instead of hanging the GPU.
+inline unsigned long long wait_timeout_ns() {
+  static const unsigned long long ns = [] {
+    const char* e = std::getenv("MLXB200_P2P_TIMEOUT_S");
+    const double sec = (e != nullptr && std::atof(e) > 0.0) ? std::atof(e) : 20.0;
+    return static_cast<unsigned long long>(sec * 1e9);
+  }();
+  return ns;
+}
+
 cudaError_t wait_flag_launch(const uint32_t* flag, uint32_t expected, uint32_t* error_flag, cudaStream_t s);
 // error_host (optional): mapped pinned host word set on a timeout, so the host can poll for failures without a device sync
 cudaError_t wait_flag_counter_launch(const uint32_t* flag, uint32_t* local_counter, uint32_t* error_flag, uint32_t* error_host,
@@ -135,20 +148,10 @@ cudaError_t advance_meta_launch(int* positions, int* context_lens, int* slots, c
 void pdl_skip_next();
 
 // ---- ep.cu (expert-parallel all-to-all over peer memory)
-cudaError_t ep_dispatch_launch(const void* x, long long ld_x, const int* idx, int npairs, int top_k, int H, int experts_per_rank,
-                               int world, int my_rank, int cap, const unsigned long long* recv_x, const unsigned long long* recv_meta,
-                               const unsigned long long* recv_count, uint32_t* send_seq, int* send_counts,
-                               unsigned int* done_counter, uint32_t* ret_expected, cudaStream_t s);
-// v2: sender-side slot reservation into the destination's expert-major buffer (no regroup kernels on the receive side)
-cudaError_t ep_dispatch_scatter_launch(const void* x, long long ld_x, const int* idx, int npairs, int top_k, int H, int experts_per_rank,
-                                       int world, int my_rank, int cap_e, const unsigned long long* recv_x,
-                                       const unsigned long long* recv_dst, const unsigned long long* recv_cnt,
-                                       const unsigned long long* recv_seq, const unsigned long long* my_ret, uint32_t* send_seq,
-                                       unsigned int* done_counter, uint32_t* ret_expected, cudaStream_t s);
-cudaError_t ep_regroup_launch(const unsigned long long* recv_words, uint32_t* local_counter, uint32_t* error_flag, int* recv_count,
-                              const void* recv_meta, const void* recv_x, int world, int cap, int E_local, int H, int* expert_offsets,
-                              int* row_perm, int* total_rows, void* x_perm, const unsigned long long* ret_y,
-                              unsigned long long* row_dst, cudaStream_t s);
+// sender-side slot reservation into every destination's expert-major receive buffer, then the step's publication
+cudaError_t ep_dispatch_scatter_launch(const void* x, long long ld_x, const int* idx, int npairs, int top_k, int H, const EpDispatch& ep,
+                                       cudaStream_t s);
+// wait for every rank's returned rows (bounded by wait_timeout_ns), then the weighted combine (+ residual, + the next norm)
 cudaError_t ep_combine_launch(const uint32_t* flag, const uint32_t* expected_ptr, uint32_t* error_flag, const float* ret_y,
                               const float* wts, const void* residual, long long ld_res, void* out, long long ld_out, int T, int top_k,
                               int H, cudaStream_t s, const void* norm_w = nullptr, float norm_eps = 0.f,

@@ -2,6 +2,7 @@
 // top-k), token permutation for the grouped GEMM, and the weighted combine fused with the residual and
 // — on the last layer of a stage — with the P2P hand-off flag.  The reference gets this from
 // mlx_lm's MoEGate + SwitchGLU (`mx.gather_qmm`, `(y * scores[..., None]).sum(-2)`); nothing is ported.
+#include "ep_dispatch.cuh"
 #include "kernels.h"
 #include "launch.h"
 #include "ptx.cuh"
@@ -40,7 +41,7 @@ __global__ void __launch_bounds__(kRouteToks == 1 ? 1024 : kRouteThreads)
 moe_route_kernel(const __nv_bfloat16* __restrict__ x, long long ld_x, const __nv_bfloat16* __restrict__ gw, int T, int H,
                  int E, int top_k, int n_group, int topk_group, float scaling, int norm_topk, int extra, int* __restrict__ idx,
                  float* __restrict__ wts, int* __restrict__ sc_counts, int sc_stride, int* __restrict__ sc_pair_row,
-                 __nv_bfloat16* __restrict__ sc_x, const __nv_bfloat16* __restrict__ norm_w, float norm_eps, const RouteEP ep,
+                 __nv_bfloat16* __restrict__ sc_x, const __nv_bfloat16* __restrict__ norm_w, float norm_eps, const EpDispatch ep,
                  __nv_bfloat16* __restrict__ normed_out, long long ld_normed) {
   pdl_sync();  // PDL: predecessor's writes visible; let the successor start its prologue
   // expert-parallel dispatch fused into the router: this step's sequence number (bumped by the last CTA at the very end, after
@@ -229,12 +230,8 @@ moe_route_kernel(const __nv_bfloat16* __restrict__ x, long long ld_x, const __nv
     // sender-side slot reservation in the owner's expert-major receive buffer (counters double-buffered by step parity) + the
     // address the owner's down-projection epilogue returns this pair's output row to (my return buffer as mapped by the owner)
     const int dst = my_i / ep.experts_per_rank, le = my_i - dst * ep.experts_per_rank;
-    const int slot = atomicAdd_system(reinterpret_cast<int*>(ep.recv_cnt.p[dst]) + (int)(ep_seq & 1u) * ep.experts_per_rank + le, 1);
-    const int r = slot < ep.cap_e ? le * ep.cap_e + slot : -1;
-    s_rows[lane] = r;
+    s_rows[lane] = ep_reserve_row(ep, ep_seq, dst, le, (unsigned long long)t * top_k + lane, H);
     s_dst[lane] = dst;
-    if (r >= 0)
-      reinterpret_cast<unsigned long long*>(ep.recv_dst.p[dst])[r] = ep.my_ret.p[dst] + ((unsigned long long)t * top_k + lane) * H * sizeof(float);
   }
   }
   if (kRouteToks == 1 && sc_counts != nullptr) {
@@ -256,24 +253,7 @@ moe_route_kernel(const __nv_bfloat16* __restrict__ x, long long ld_x, const __nv
           reinterpret_cast<uint4*>(ep.recv_x.p[s_dst[k]])[(size_t)s_rows[k] * nvec + v] = reinterpret_cast<const uint4*>(xs)[v];
       }
     }
-    // publication (same protocol as ep_dispatch_scatter_kernel): every CTA fences its remote stores, the last one writes the
-    // step's sequence number to every destination with release.sys and advances the local step state
-    __threadfence_system();
-    __syncthreads();
-    __shared__ bool last;
-    if (threadIdx.x == 0) last = (atomicAdd(ep.done_counter, 1u) + 1u == gridDim.x);
-    __syncthreads();
-    if (last) {
-      __threadfence_system();
-      for (int r = threadIdx.x; r < ep.world; r += blockDim.x)
-        st_release_sys_u64(reinterpret_cast<unsigned long long*>(ep.recv_seq.p[r]) + ep.my_rank, (unsigned long long)ep_seq);
-      __syncthreads();
-      if (threadIdx.x == 0) {
-        *ep.send_seq = ep_seq;
-        *ep.done_counter = 0u;
-        if (ep.ret_expected != nullptr) *ep.ret_expected += (uint32_t)ep.world;
-      }
-    }
+    ep_publish(ep, ep_seq);
   }
 }
 
@@ -472,8 +452,8 @@ moe_combine_norm_kernel(const float* __restrict__ y_perm, const int* __restrict_
 cudaError_t moe_route_launch(const void* x, long long ld_x, const void* gate_w, int T, int H, int E, int top_k, int n_group,
                              int topk_group, float scaling, bool norm_topk, int extra, int* idx, float* wts, int* sc_counts,
                              int sc_stride, int* sc_pair_row, void* sc_x, const void* norm_w, float norm_eps, cudaStream_t s,
-                             const RouteEP* ep_in, void* normed_out, long long ld_normed) {
-  RouteEP ep;
+                             const EpDispatch* ep_in, void* normed_out, long long ld_normed) {
+  EpDispatch ep;
   if (ep_in != nullptr) ep = *ep_in;
   if (ep.enabled && (T == 0 || T > 1024 || ep.world > kEpMaxWorld || sc_counts != nullptr)) return cudaErrorInvalidValue;   // one-token-per-CTA variant only
   if (T == 0) return cudaSuccess;

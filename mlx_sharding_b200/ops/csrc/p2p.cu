@@ -3,8 +3,6 @@
 // cannot ride a GEMM epilogue, and the on-device step-metadata advance that lets a CUDA-graphed decode
 // step re-run without any host -> device traffic.  The reference's equivalent is a blocking gRPC unary
 // call per stage per token with host staging (shard/utils.py:71-90,162-164).
-#include <cstdlib>
-
 #include "kernels.h"
 #include "launch.h"
 #include "ptx.cuh"
@@ -12,12 +10,6 @@
 namespace b200 {
 
 namespace {
-
-__device__ __forceinline__ unsigned long long globaltimer_ns() {
-  unsigned long long t;
-  asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
-  return t;
-}
 
 // Spin until *flag >= expected (monotonic step counters).  Bounded: after ~timeout the kernel records an
 // error and returns instead of hanging the GPU (a dead peer must never wedge the box).
@@ -95,16 +87,6 @@ __global__ void advance_meta_kernel(int* positions, int* context_lens, int* slot
 }
 
 }  // namespace
-
-// bounded spin of the flag waits: MLXB200_P2P_TIMEOUT_S (default 20 s)
-static unsigned long long wait_timeout_ns() {
-  static const unsigned long long ns = [] {
-    const char* e = std::getenv("MLXB200_P2P_TIMEOUT_S");
-    const double sec = (e != nullptr && std::atof(e) > 0.0) ? std::atof(e) : 20.0;
-    return static_cast<unsigned long long>(sec * 1e9);
-  }();
-  return ns;
-}
 
 cudaError_t wait_flag_launch(const uint32_t* flag, uint32_t expected, uint32_t* error_flag, cudaStream_t s) {
   (void)launch_pdl(wait_flag_kernel, dim3(1), dim3(1), 0, s, flag, expected, error_flag, wait_timeout_ns());

@@ -209,6 +209,23 @@ B200_DEVICE uint32_t ld_acquire_gpu(const uint32_t* p) {
   asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
   return v;
 }
+B200_DEVICE unsigned long long globaltimer_ns() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
+  return t;
+}
+// Bounded acquire spin: polls `ready()` (an acquire load of a word another rank releases) until it holds.  Once `timeout_ns` have
+// passed since `t0` it sets *error (when given) and returns, so a lost peer becomes an error word the host reads, not a hung GPU.
+template <typename Ready>
+B200_DEVICE void spin_acquire(Ready ready, unsigned long long t0, unsigned long long timeout_ns, uint32_t* error) {
+  while (!ready()) {
+    if (globaltimer_ns() - t0 > timeout_ns) {
+      if (error != nullptr) atomicExch(error, 1u);
+      return;
+    }
+    __nanosleep(32);
+  }
+}
 B200_DEVICE void named_bar_sync(uint32_t id, uint32_t nthreads) {
   asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(nthreads) : "memory");
 }

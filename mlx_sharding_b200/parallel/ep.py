@@ -23,11 +23,14 @@ from ..ops.weights import LinearWeight
 
 
 class EPBuffers:
-    """IPC-mapped receive / return buffers of one rank (shared by all MoE layers of that rank)."""
+    """IPC-mapped receive / return buffers of one rank (shared by all MoE layers of that rank).
 
-    def __init__(self, hidden: int, max_tokens: int, top_k: int, group=None, experts_per_rank: int = 0):
-        import os
+    Layout of the mapped region: ``[E_local][world * max_tokens][H]`` bf16 receive rows (expert-major, written by the senders) |
+    their return addresses (u64) | ``[2][E_local]`` int32 row counters (double-buffered by step parity) | one u64 arrival word per
+    source (the step's sequence number, released by the source's dispatch) | the fp32 return rows of this rank's own pairs |
+    flags (the return flag every destination's down-projection bumps)."""
 
+    def __init__(self, hidden: int, max_tokens: int, top_k: int, experts_per_rank: int, group=None):
         from ..ops import b200
 
         self.C = b200.load_extension()
@@ -35,24 +38,17 @@ class EPBuffers:
         self.dev = torch.cuda.current_device()
         self.H, self.top_k = hidden, top_k
         self.max_tokens = max_tokens
-        # v2 (default): sender-side slot reservation into an expert-major receive buffer, no regroup kernels (ops/csrc/ep.cu)
-        self.v2 = experts_per_rank > 0 and os.environ.get("MLXB200_EP_V2", "1") != "0"
         self.E_local = experts_per_rank
-        self.cap = max_tokens * top_k                      # rows one source can send to one destination
+        self.cap = max_tokens * top_k                      # pairs one rank can route per step
         W, cap, H = self.world, self.cap, hidden
+        rows = experts_per_rank * W * max_tokens
         self.off_recv_x = 0
-        if self.v2:
-            # [E_local][W * max_tokens][H] rows + their return addresses (u64) + [2][E_local] counters; arrival words live in the
-            # recv_count slot
-            rows = experts_per_rank * W * max_tokens
-            self.off_recv_meta = self.off_recv_x + rows * H * 2            # -> row_dst table
-            self.off_cnt = self.off_recv_meta + rows * 8
-            self.off_recv_count = (self.off_cnt + 2 * experts_per_rank * 4 + 255) // 256 * 256
-        else:
-            self.off_recv_meta = self.off_recv_x + W * cap * H * 2
-            self.off_recv_count = self.off_recv_meta + W * cap * 8
-        self.off_ret_y = (self.off_recv_count + W * 8 + 255) // 256 * 256     # recv_count: one u64 (count << 32 | step seq) per source
+        self.off_row_dst = self.off_recv_x + rows * H * 2
+        self.off_cnt = self.off_row_dst + rows * 8
+        self.off_arrive = (self.off_cnt + 2 * experts_per_rank * 4 + 255) // 256 * 256
+        self.off_ret_y = (self.off_arrive + W * 8 + 255) // 256 * 256
         self.off_flags = self.off_ret_y + cap * H * 4
+        self.off_ret_flag = self.off_flags + 128
         total = self.off_flags + 256
         self.base, handle = self.C.ipc_alloc(total)
         handles: List = [None] * W
@@ -65,42 +61,53 @@ class EPBuffers:
                 if pdev != self.dev:
                     self.C.enable_peer_access(pdev)
                 self.peer.append(self.C.ipc_open(h))
-        # tables of peer addresses
+        # tables of peer addresses, one per rank
         self.t_recv_x = [p + self.off_recv_x for p in self.peer]
-        self.t_recv_meta = [p + self.off_recv_meta for p in self.peer]
-        self.t_recv_count = [p + self.off_recv_count for p in self.peer]
-        self.t_ret_y = [p + self.off_ret_y for p in self.peer]
-        self.t_ret_flag = [p + self.off_flags + 128 for p in self.peer]
-        if self.v2:
-            self.t_cnt = [p + self.off_cnt for p in self.peer]
-            # my return buffer as mapped by every destination (the address a destination's down-projection epilogue stores to)
-            peers_all: List = [None] * W
-            dist.all_gather_object(peers_all, list(self.peer), group=group)
-            self.t_my_ret = [peers_all[d][self.rank] + self.off_ret_y for d in range(W)]
-            self.cnt = self.C.tensor_from_ptr(self.base + self.off_cnt, [2 * experts_per_rank], "int32", self.dev)
-            self._views = {}
-        # device-resident local state: [send_counts(world) | dispatch done ctr | down-GEMM tile ctr | regroup step seq seen |
-        #                               return arrivals expected | dispatch step seq | ... | error]
-        self.state = torch.zeros(W + 8, dtype=torch.int32, device="cuda")
+        self.t_row_dst = [p + self.off_row_dst for p in self.peer]
+        self.t_cnt = [p + self.off_cnt for p in self.peer]
+        self.t_arrive = [p + self.off_arrive for p in self.peer]
+        # my return buffer as mapped by every destination (the address a destination's down-projection epilogue stores to)
+        peers_all: List = [None] * W
+        dist.all_gather_object(peers_all, list(self.peer), group=group)
+        self.t_my_ret = [peers_all[d][self.rank] + self.off_ret_y for d in range(W)]
+        self.cnt = self.C.tensor_from_ptr(self.base + self.off_cnt, [2 * experts_per_rank], "int32", self.dev)
+        self.arrive = self.base + self.off_arrive          # the W arrival words the grouped gate/up GEMM acquires
+        self.ret_flag = self.base + self.off_ret_flag      # my return flag, bumped by every destination's down-projection
+        self.ret_flags_dev = torch.tensor([p + self.off_ret_flag for p in self.peer], dtype=torch.int64, device="cuda")
+        self._views = {}
+        # device-resident step state; every field is a one-element view, passed to the kernels by pointer
+        self.state = torch.zeros(5, dtype=torch.int32, device="cuda")
+        self.send_seq = self.state[0:1]          # dispatch step sequence number (also what the arrival wait expects)
+        self.done_counter = self.state[1:2]      # dispatch CTAs arrived (the last one publishes)
+        self.down_tiles = self.state[2:3]        # down-projection tiles stored (the last CTA signals every source)
+        self.ret_expected = self.state[3:4]      # return-flag value the combine of this step waits for
+        self.error_word = self.state[4:5]        # set by any wait that times out
+        self.error_ptr = self.error_word.data_ptr()
         self.ret_y = self.C.tensor_from_ptr(self.base + self.off_ret_y, [cap, H], "float32", self.dev)
-        self.ret_flags_dev = torch.tensor(self.t_ret_flag, dtype=torch.int64, device="cuda")   # every source's return flag
         dist.barrier(group=group)
 
     def error(self) -> bool:
-        return bool(self.state[-1].item())
+        return bool(self.error_word.item())
 
     def recv_views(self, stride: int):
-        """(rows [E_local * stride, H] bf16, row_dst [E_local * stride] int64) over the v2 receive buffer for this step's stride."""
+        """(rows [E_local * stride, H] bf16, row_dst [E_local * stride] int64) over the receive buffer for this step's stride."""
         v = self._views.get(stride)
         if v is None:
             R = self.E_local * stride
             v = self._views[stride] = (self.C.tensor_from_ptr(self.base + self.off_recv_x, [R, self.H], "bfloat16", self.dev),
-                                       self.C.tensor_from_ptr(self.base + self.off_recv_meta, [R], "int64", self.dev))
+                                       self.C.tensor_from_ptr(self.base + self.off_row_dst, [R], "int64", self.dev))
         return v
+
+    def dispatch_args(self, stride: int):
+        """Arguments of both dispatch launches after ``experts_per_rank, my_rank``: receive stride, peer tables, step state."""
+        return (stride, self.t_recv_x, self.t_row_dst, self.t_cnt, self.t_arrive, self.t_my_ret, self.send_seq, self.done_counter,
+                self.ret_expected)
 
 
 class ExpertParallelMoE:
-    """One MoE layer's routed experts, sharded over the ranks of ``bufs``."""
+    """One MoE layer's routed experts, sharded over the ranks of ``bufs``.  A step is four launches: dispatch (slot reservation at
+    the sender; on its own, or folded into the router by ``route_forward``) -> grouped gate/up GEMM (acquires the arrivals itself)
+    -> grouped down GEMM (its epilogue returns the rows) -> combine."""
 
     def __init__(self, bufs: EPBuffers, Wg: LinearWeight, Wu: LinearWeight, Wd: LinearWeight, num_experts: int,
                  act: str = "silu", weights_are_local: bool = False):
@@ -116,113 +123,73 @@ class ExpertParallelMoE:
         self.wg, self.wu, self.wd = pick(Wg), pick(Wu), pick(Wd)
         self.act = b200.ACT_IDS[act]
 
+    def _stride(self, Tmax: int) -> int:
+        """Receive rows per expert this step: ``world * Tmax`` rounded up to 64 (every rank computes the same value: ranks step in
+        lock-step with equal batch shapes, or pass ``peer_tokens``)."""
+        b = self.b
+        return min(b.world * b.max_tokens, (b.world * Tmax + 63) // 64 * 64)
+
     def forward(self, x: torch.Tensor, idx: torch.Tensor, w: torch.Tensor, residual: Optional[torch.Tensor] = None,
                 out: Optional[torch.Tensor] = None, peer_tokens: Optional[int] = None, join=None) -> torch.Tensor:
         """``peer_tokens``: upper bound of the tokens *any* rank routes in this step (default: this rank's own ``T`` —
-        ranks stepping in lockstep with equal batch shapes); only sizes the temporaries of the local expert GEMMs."""
-        b, C = self.b, self.b.C
+        ranks stepping in lockstep with equal batch shapes); only sizes the receive stride and the local expert GEMMs."""
+        b = self.b
         T, k = idx.shape
         assert T * k <= b.cap, "token batch exceeds the EP buffer capacity"
-        W = b.world
-        st = b.state
         Tmax = max(T, peer_tokens or getattr(self, "peer_tokens_default", 0) or 0)
-        if b.v2:
-            return self._forward_v2(x, idx, w, residual, out, Tmax, join)
-        # 1) dispatch my pairs to the owners of their experts (remote stores + count/flag publication); also advances the
-        #    arrival target of this step's combine (st[W+3] += world)
-        C.ep_dispatch(x, idx, self.E_local, b.rank, b.cap, b.t_recv_x, b.t_recv_meta, b.t_recv_count, st[W + 4:W + 5],
-                      st[:W], st[W:W + 1], st[W + 3:W + 4])
-        # 2) wait for every source, bucket what I received by local expert; row_dst[r] = where row r's output must go
-        offs, total, x_perm, row_dst = C.ep_regroup(
-            b.base + b.off_recv_count, st[W + 2:W + 3].data_ptr(), st[-1:].data_ptr(),
-            b.base + b.off_recv_meta, b.base + b.off_recv_x, W, b.cap, self.E_local, b.H, b.dev, min(W * b.cap, W * Tmax * k), b.t_ret_y)
-        # 3) my experts: grouped swap-AB wgmma GEMMs on the received rows; the down-projection epilogue stores every output
-        #    row straight into its source rank's return buffer (peer memory) and the last tile bumps all sources' flags
-        max_rows = min(W * Tmax, x_perm.shape[0])  # upper bound of rows one expert can receive (every rank sends <= Tmax)
-        exp_rows = T * k  # balanced routing: a rank receives about as many pairs as it sends (only picks the token tile size)
-        h = C.grouped_linear(x_perm, self.wg, self.wu, offs, max_rows, self.act, False, None, None, None, exp_rows)
-        C.grouped_linear(h, self.wd, None, offs, max_rows, 0, True, row_dst, b.ret_flags_dev, st[W + 1:W + 2], exp_rows)
-        # 4) wait for all my pairs to come home + weighted combine (+ residual): one kernel
+        stride = self._stride(Tmax)
+        b.C.ep_dispatch_scatter(x, idx, self.E_local, b.rank, *b.dispatch_args(stride))
+        return self._experts_and_combine(T * k, Tmax, stride, w, residual, out, join)
+
+    def route_forward(self, h, gate_w, route_kw: dict, pre_norm, residual_fn, out=None, next_norm=None):
+        """The whole expert-parallel block as FOUR kernels (1 <= T <= 1024): router with the pre-MoE RMSNorm and the dispatch
+        folded in (``moe.cu``: the token's CTA reserves its pairs' slots on the owners with remote atomics, stores the normalised
+        row there and takes part in the publication) -> grouped gate/up GEMM -> grouped down GEMM -> combine with the next layer's
+        input norm folded in.
+
+        ``h``: un-normalised residual stream; ``pre_norm = (weight, eps)``; ``residual_fn(normed)`` -> ``(residual, join)``: called
+        right after the router so the shared-expert branch (which consumes ``normed``) forks onto the side stream behind it;
+        ``next_norm = (weight, eps)`` or None.  Returns ``out`` or ``(out, normed_next)``."""
+        b, C = self.b, self.b.C
+        from ..ops import b200 as O
+
+        T = h.shape[0]
+        k = int(route_kw["top_k"])
+        assert 1 <= T <= 1024 and T * k <= b.cap
+        Tmax = max(T, getattr(self, "peer_tokens_default", 0) or 0)
+        stride = self._stride(Tmax)
+        rk = dict(route_kw)
+        if rk.pop("method", "greedy") != "group_limited_greedy":
+            rk["n_group"], rk["topk_group"] = 1, 1
+        normed = torch.empty_like(h)
+        idx, w = C.ep_route_dispatch(h, O._bf16(gate_w), k, int(rk["n_group"]), int(rk["topk_group"]), float(rk["scaling"]),
+                                     bool(rk["norm_topk"]), self.E_local, b.rank, *b.dispatch_args(stride),
+                                     O._bf16(pre_norm[0]), float(pre_norm[1]), normed)
+        residual, join = residual_fn(normed)
+        fuse_norm = next_norm is not None and h.shape[1] <= 8192
+        nxt = torch.empty_like(h) if fuse_norm else None
+        res = self._experts_and_combine(T * k, Tmax, stride, w, residual, out, join, next_norm if fuse_norm else None, nxt)
+        if next_norm is None:
+            return res
+        return res, (nxt if fuse_norm else O.rmsnorm(res, next_norm[0], next_norm[1]))
+
+    def _experts_and_combine(self, npairs, Tmax, stride, w, residual, out, join, norm=None, normed=None):
+        """Grouped gate/up (waits for every source's arrival word) -> grouped down (its epilogue stores each output row into the
+        source's return buffer and the last CTA bumps every source's return flag) -> combine (waits for all returns; + residual,
+        + ``norm = (weight, eps)`` into ``normed``)."""
+        b, C = self.b, self.b.C
+        rows, row_dst = b.recv_views(stride)
+        max_rows = min(b.world * Tmax, stride)   # upper bound of rows one expert can receive (every rank sends <= Tmax)
+        exp_rows = npairs                        # balanced routing: a rank receives about as many pairs as it sends
+        wait = (stride, b.arrive, b.send_seq, b.error_ptr, b.world)
+        h = C.grouped_linear(rows, self.wg, self.wu, b.cnt, max_rows, self.act, False, None, None, None, exp_rows, *wait, True)
+        C.grouped_linear(h, self.wd, None, b.cnt, max_rows, 0, True, row_dst, b.ret_flags_dev, b.down_tiles, exp_rows, *wait, False)
         if join is not None:
-            join.wait()  # ``residual`` (shared-expert branch) is produced on the side stream
-        return C.ep_combine(b.base + b.off_flags + 128, st[W + 3:W + 4], st[-1:].data_ptr(), b.ret_y, w, residual, out)
-
-
-    # (method of ExpertParallelMoE; placed after forward for readability)
-    pass
-
-
-def _forward_v2(self, x, idx, w, residual, out, Tmax, join):
-    """v2 exchange: 4 launches — dispatch (slot reservation at the sender) -> grouped gate/up GEMM (acquires the arrivals itself) ->
-    grouped down GEMM (epilogue returns the rows) -> combine.  The receive stride of this step is ``world * Tmax`` rows per expert
-    (every rank computes the same value: ranks step in lock-step with equal batch shapes, or pass ``peer_tokens``)."""
-    b, C = self.b, self.b.C
-    T, k = idx.shape
-    W, st = b.world, b.state
-    stride = min(W * b.max_tokens, (W * Tmax + 63) // 64 * 64)
-    rows, row_dst = b.recv_views(stride)
-    C.ep_dispatch_scatter(x, idx, self.E_local, b.rank, stride, b.t_recv_x, b.t_recv_meta, b.t_cnt, b.t_recv_count, b.t_my_ret,
-                          st[W + 4:W + 5], st[W:W + 1], st[W + 3:W + 4])
-    max_rows = min(W * Tmax, stride)
-    exp_rows = T * k
-    arrive, seq, err = b.base + b.off_recv_count, st[W + 4:W + 5], st[-1:].data_ptr()
-    h = C.grouped_linear(rows, self.wg, self.wu, b.cnt, max_rows, self.act, False, None, None, None, exp_rows, stride, arrive, seq, err, W, True)
-    C.grouped_linear(h, self.wd, None, b.cnt, max_rows, 0, True, row_dst, b.ret_flags_dev, st[W + 1:W + 2], exp_rows, stride, arrive, seq, err,
-                     W, False)
-    if join is not None:
-        join.wait()
-    return C.ep_combine(b.base + b.off_flags + 128, st[W + 3:W + 4], st[-1:].data_ptr(), b.ret_y, w, residual, out)
-
-
-ExpertParallelMoE._forward_v2 = _forward_v2
-
-
-def _route_forward(self, h, gate_w, route_kw: dict, pre_norm, residual_fn, out=None, next_norm=None):
-    """The whole expert-parallel block as FOUR kernels (v2 exchange, 1 <= T <= 1024): router with the pre-MoE RMSNorm and the
-    dispatch folded in (``moe.cu``: the token's CTA reserves its pairs' slots on the owners with remote atomics, stores the
-    normalised row there and takes part in the publication) -> grouped gate/up GEMM (acquires the arrivals) -> grouped down GEMM
-    (epilogue returns the rows) -> combine with the next layer's input norm folded in.
-
-    ``h``: un-normalised residual stream; ``pre_norm = (weight, eps)``; ``residual_fn(normed)`` -> ``(residual, join)``: called
-    right after the router so the shared-expert branch (which consumes ``normed``) forks onto the side stream behind it;
-    ``next_norm = (weight, eps)`` or None.  Returns ``out`` or ``(out, normed_next)``."""
-    b, C = self.b, self.b.C
-    from ..ops import b200 as O
-
-    T = h.shape[0]
-    k = int(route_kw["top_k"])
-    assert b.v2 and 1 <= T <= 1024 and T * k <= b.cap
-    W, st = b.world, b.state
-    Tmax = max(T, getattr(self, "peer_tokens_default", 0) or 0)
-    stride = min(W * b.max_tokens, (W * Tmax + 63) // 64 * 64)
-    rows, row_dst = b.recv_views(stride)
-    rk = dict(route_kw)
-    if rk.pop("method", "greedy") != "group_limited_greedy":
-        rk["n_group"], rk["topk_group"] = 1, 1
-    normed = torch.empty_like(h)
-    idx, w = C.ep_route_dispatch(h, O._bf16(gate_w), k, int(rk["n_group"]), int(rk["topk_group"]), float(rk["scaling"]),
-                                 bool(rk["norm_topk"]), self.E_local, b.rank, stride, b.t_recv_x, b.t_recv_meta, b.t_cnt,
-                                 b.t_recv_count, b.t_my_ret, st[W + 4:W + 5], st[W:W + 1], st[W + 3:W + 4],
-                                 O._bf16(pre_norm[0]), float(pre_norm[1]), normed)
-    residual, join = residual_fn(normed)
-    max_rows = min(W * Tmax, stride)
-    exp_rows = T * k
-    arrive, seq, err = b.base + b.off_recv_count, st[W + 4:W + 5], st[-1:].data_ptr()
-    hmid = C.grouped_linear(rows, self.wg, self.wu, b.cnt, max_rows, self.act, False, None, None, None, exp_rows, stride, arrive, seq, err, W, True)
-    C.grouped_linear(hmid, self.wd, None, b.cnt, max_rows, 0, True, row_dst, b.ret_flags_dev, st[W + 1:W + 2], exp_rows, stride, arrive, seq, err,
-                     W, False)
-    if join is not None:
-        join.wait()
-    flag, exp, errp = b.base + b.off_flags + 128, st[W + 3:W + 4], st[-1:].data_ptr()
-    if next_norm is not None and h.shape[1] <= 8192:
-        nxt = torch.empty_like(h)
-        res = C.ep_combine(flag, exp, errp, b.ret_y, w, residual, out, O._bf16(next_norm[0]), float(next_norm[1]), nxt)
-        return res, nxt
-    res = C.ep_combine(flag, exp, errp, b.ret_y, w, residual, out)
-    return res if next_norm is None else (res, O.rmsnorm(res, next_norm[0], next_norm[1]))
-
-
-ExpertParallelMoE.route_forward = _route_forward
+            join.wait()   # ``residual`` (shared-expert branch) is produced on the side stream
+        if norm is None:
+            return C.ep_combine(b.ret_flag, b.ret_expected, b.error_ptr, b.ret_y, w, residual, out)
+        return C.ep_combine(b.ret_flag, b.ret_expected, b.error_ptr, b.ret_y, w, residual, out, self.ops._bf16(norm[0]),
+                            float(norm[1]), normed)
 
 
 class ExpertParallelMoERef:
@@ -299,8 +266,7 @@ def enable_expert_parallel(model, max_tokens: int = 256, group=None):
         model.unfuse_shared_experts()     # shared experts were appended to the (un-sharded) routed bank: split them off again
     fused = model.backend_name == "b200"
     world = dist.get_world_size(group)
-    bufs = EPBuffers(cfg.hidden_size, max_tokens, cfg.num_experts_per_tok, group=group,
-                     experts_per_rank=cfg.n_routed_experts // world) if fused else None
+    bufs = EPBuffers(cfg.hidden_size, max_tokens, cfg.num_experts_per_tok, cfg.n_routed_experts // world, group=group) if fused else None
     model.ep_layers = {}
     for i, w in model.layer_weights.items():
         if "router" not in w:

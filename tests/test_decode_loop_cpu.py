@@ -65,7 +65,9 @@ def _worker(rank, world, port, C, half, q):
     if rank == 0:
         for g in range(G):
             hist[g].append(loop.groups[g].tokens.clone())
-        q.put((prompts, [torch.stack(h) for h in hist]))
+        # numpy arrays travel by value; a tensor put on the queue is handed over as a shared-memory file descriptor, which the
+        # parent can only fetch from this process while it is alive, and it exits right after the barrier below
+        q.put((prompts.numpy(), [torch.stack(h).numpy() for h in hist]))
     dist.barrier()
     dist.destroy_process_group()
 

@@ -33,20 +33,19 @@ def test_serving_chain_parity(arch, transport, port):
     assert "SERVING_OK" in out, out[-3000:]
 
 
-@pytest.mark.parametrize("version,port", [("v2", 29574), ("v1", 29578)])
-def test_expert_parallel_moe(version, port):
-    """v2: sender-side slot reservation + arrival wait fused into the grouped GEMM; v1: regroup kernels on the receive side."""
-    out = _torchrun("ep_parity.py", [version], port=port)
-    assert "EP_OK " + version in out, out[-3000:]
+def test_expert_parallel_moe():
+    """Sender-side slot reservation, arrival wait fused into the grouped gate/up GEMM, return fused into the down GEMM's epilogue."""
+    out = _torchrun("ep_parity.py", [], port=29574)
+    assert "EP_OK" in out, out[-3000:]
 
 
-@pytest.mark.parametrize("version,port", [("v2", 29584), ("v1", 29585), ("fused", 29586)])
-def test_expert_parallel_stress(version, port):
+@pytest.mark.parametrize("mode,port", [("forward", 29584), ("fused", 29586)])
+def test_expert_parallel_stress(mode, port):
     """Several EP layers sharing one buffer set, called back to back with no host synchronisation, token counts changing from step
     to step (prefill chunk <-> decode batch), two geometries; every output must equal the local MoE bit for bit.  ``fused``: the
     four-kernel block (norm + router + dispatch in one kernel, combine + next norm in one) against separate kernels."""
-    out = _torchrun("ep_stress.py", [version], port=port)
-    assert "EP_STRESS_OK " + version in out, out[-3000:]
+    out = _torchrun("ep_stress.py", [mode], port=port)
+    assert "EP_STRESS_OK " + mode in out, out[-3000:]
 
 
 def test_expert_parallel_whole_model():
