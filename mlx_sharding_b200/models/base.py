@@ -129,7 +129,14 @@ class StageModel:
 
     # weights ---------------------------------------------------------------------------------
     def _lin(self, sd, prefix) -> LinearWeight:
-        return LinearWeight.from_state(sd, prefix, self.qcfg, dtype=self.dtype, device=self.device)
+        W = LinearWeight.from_state(sd, prefix, self.qcfg, dtype=self.dtype, device=self.device)
+        ad = getattr(self, "_adapter", None)
+        if ad and prefix in ad:
+            from ..utils.adapters import attach
+
+            A, B = ad.pop(prefix)
+            W = attach(W, prefix, A, B, ad.scale, ad.path)
+        return W
 
     def _vec(self, sd, key) -> torch.Tensor:
         return sd.pop(key).to(device=self.device, dtype=self.dtype)
@@ -140,8 +147,15 @@ class StageModel:
 
         return {k: v for k, v in sd.items() if key_in_shard(k, self.spec, self.cfg.tie_word_embeddings, self.cfg.model_type)}
 
-    def load_state(self, sd: Dict[str, torch.Tensor], strict: bool = True):
+    def load_state(self, sd: Dict[str, torch.Tensor], strict: bool = True, adapter=None):
+        """``adapter``: a LoRA adapter (``utils/adapters.py::load_adapter``); this stage applies the entries of the layers (and
+        half layers) it runs, and every such entry must reach a linear weight."""
         sd = self.sanitize(dict(sd))
+        if adapter is not None:
+            from ..utils.checkpoint import key_in_shard
+
+            adapter.check_layers(self.cfg.num_hidden_layers)
+            self._adapter = adapter.subset(lambda k: key_in_shard(k + ".lora_a", self.spec, model_type=self.cfg.model_type))
         if self.needs_embed:
             self.embed_tokens = self._lin(sd, "model.embed_tokens")
         else:
@@ -160,6 +174,10 @@ class StageModel:
                 self.lm_head = self._lin(sd, "lm_head")
         if strict and sd:
             raise ValueError(f"unexpected checkpoint tensors for stage {self.spec}: {sorted(sd)[:8]} ...")
+        left, self._adapter = getattr(self, "_adapter", None), None
+        if left:
+            raise ValueError(f"{left.path}: tensors match no linear weight of this {self.cfg.model_type} stage: "
+                             f"{[k + '.lora_a' for k in sorted(left)][:8]}")
         self.rope = self._make_rope()
         self.rope.inv_freq = self.rope.inv_freq.to(self.device)
         self._post_load()
@@ -181,7 +199,9 @@ class StageModel:
         def visit(o):
             nonlocal total
             if isinstance(o, LinearWeight):
-                for t in (o.weight, o.wq, o.scales, o.biases, o.bias) + tuple(getattr(o, "_fp8", None) or ()):
+                # (+ the concatenated A of an adapted gate/up pair, ops/b200.py::_lora_pair, once built)
+                for t in ((o.weight, o.wq, o.scales, o.biases, o.bias, o.lora_a, o.lora_b_scaled) + tuple(getattr(o, "_fp8", None) or ())
+                          + tuple(getattr(o, "_lora_pair", ())[1:])):
                     if t is not None and t.data_ptr() not in seen:
                         seen.add(t.data_ptr())
                         total += t.numel() * t.element_size()

@@ -65,7 +65,7 @@ def _bf16(t: torch.Tensor) -> torch.Tensor:
 def _dense(W: LinearWeight) -> torch.Tensor:
     """bf16 ``[.., N, K]`` view of a weight.  Only used for bf16 checkpoints and for quantised layouts the in-kernel
     dequant GEMM does not cover (2-bit, odd group sizes; expert-parallel banks): those are expanded once at
-    first use.  int4 / int8 group-64/128 weights take :func:`_qpack` and stay packed in HBM."""
+    first use, with their LoRA adapter folded in.  int4 / int8 group-64/128 weights take :func:`_qpack` and stay packed in HBM."""
     if W.is_quantized:
         if W.weight is None:
             W.weight = W.dense(torch.bfloat16).contiguous()
@@ -138,8 +138,12 @@ def linear(x: torch.Tensor, W: LinearWeight, residual: Optional[torch.Tensor] = 
     flag, val = signal if signal is not None else (0, 0)
     q = _qpack(W)
     if q is not None:
+        lk = {}
+        if W.has_lora:
+            # unfused LoRA on the packed weight: u = x A^T (lora_shrink), then the GEMM epilogue adds u B_s^T
+            lk = dict(lora_u=C().lora_shrink(x, W.lora_a), lora_b=W.lora_b_scaled)
         return C().linear_q(x, q[0], q[1], q[2], None, None, None, W.bits, W.group_size, W.out_features, residual, W.bias, 0,
-                            float(softcap), fp32, out, 0, int(flag), int(val))
+                            float(softcap), fp32, out, 0, int(flag), int(val), **lk)
     return C().linear(x, _dense(W), None, residual, W.bias, 0, float(softcap), fp32, out, 0, int(flag), int(val))
 
 
@@ -148,9 +152,36 @@ def gated_up(x: torch.Tensor, Wg: LinearWeight, Wu: LinearWeight, act: str = "si
         raise NotImplementedError("gated MLP with bias")
     qg, qu = _qpack(Wg), _qpack(Wu)
     if qg is not None and qu is not None:
+        lk = {}
+        if Wg.has_lora or Wu.has_lora:
+            a, bg, bu = _lora_pair(Wg, Wu)
+            lk = dict(lora_u=C().lora_shrink(x, a), lora_b=bg, lora_b2=bu)
         return C().linear_q(x, qg[0], qg[1], qg[2], qu[0], qu[1], qu[2], Wg.bits, Wg.group_size, Wg.out_features, None, None,
-                            ACT_IDS[act], 0.0, False, None, 0, 0, 0)
+                            ACT_IDS[act], 0.0, False, None, 0, 0, 0, **lk)
     return C().linear(x, _dense(Wg), _dense(Wu), None, None, ACT_IDS[act], 0.0, False, None, 0, 0, 0)
+
+
+def _lora_pair(Wg: LinearWeight, Wu: LinearWeight):
+    """Gate/up pair: one shrink over ``[A_g; A_u]`` (both at the same rank R) gives u [T, 2R]; the epilogue adds u[:, :R] B_g^T
+    to the gate accumulator and u[:, R:] B_u^T to the up accumulator.  Built once per pair: the concatenated A, plus zero-padded
+    copies only of a B whose rank is below R (or that has no adapter)."""
+    c = getattr(Wg, "_lora_pair", None)
+    if c is None or c[0] is not Wu:
+        r = max(w.lora_a.shape[0] for w in (Wg, Wu) if w.has_lora)   # multiples of 8 (utils/adapters.py::attach)
+
+        def at_rank(W):
+            if W.has_lora and W.lora_a.shape[0] == r:
+                return W.lora_a, W.lora_b_scaled
+            a = torch.zeros(r, W.in_features, dtype=torch.bfloat16, device=W.device)
+            b = torch.zeros(W.out_features, r, dtype=torch.bfloat16, device=W.device)
+            if W.has_lora:
+                a[: W.lora_a.shape[0]] = W.lora_a
+                b[:, : W.lora_b_scaled.shape[1]] = W.lora_b_scaled
+            return a, b
+
+        (ag, bg), (au, bu) = at_rank(Wg), at_rank(Wu)
+        c = Wg._lora_pair = (Wu, torch.cat([ag, au]).contiguous(), bg, bu)
+    return c[1:]
 
 
 def rope_(x: torch.Tensor, positions: torch.Tensor, spec: RopeSpec, rot_offset: int = 0) -> torch.Tensor:

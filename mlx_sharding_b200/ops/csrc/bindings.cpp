@@ -168,7 +168,8 @@ void check_q(const Tensor& wq, const Tensor& st, const Tensor& bt, int64_t rows,
 Tensor linear_q(const Tensor& x, const Tensor& wq, const Tensor& scales_t, const Tensor& biases_t, const c10::optional<Tensor>& wq2,
                 const c10::optional<Tensor>& scales2_t, const c10::optional<Tensor>& biases2_t, int64_t bits, int64_t group, int64_t N,
                 const c10::optional<Tensor>& residual, const c10::optional<Tensor>& bias, int64_t act, double softcap, bool out_fp32,
-                const c10::optional<Tensor>& out_, int64_t splits, int64_t signal_flag_ptr, int64_t signal_value) {
+                const c10::optional<Tensor>& out_, int64_t splits, int64_t signal_flag_ptr, int64_t signal_value,
+                const c10::optional<Tensor>& lora_u, const c10::optional<Tensor>& lora_b, const c10::optional<Tensor>& lora_b2) {
   check_bf16(x, "x"); check_rows(x, "x");
   const c10::cuda::CUDAGuard guard(x.device());
   const int64_t K = x.size(1);
@@ -179,6 +180,20 @@ Tensor linear_q(const Tensor& x, const Tensor& wq, const Tensor& scales_t, const
   if (wq2.has_value()) {
     check_q(*wq2, *scales2_t, *biases2_t, N, K, bits, group);
     a.w2 = wq2->data_ptr(); a.q_scales2_t = scales2_t->data_ptr(); a.q_biases2_t = biases2_t->data_ptr();
+  }
+  if (lora_b.has_value()) {
+    // LoRA adapter: u = x A^T from lora_shrink (fp32 [T, R], a pair's [T, 2R]), B = scale * B as bf16 [N, R] per weight
+    check_bf16(*lora_b, "lora_b");
+    const int64_t R = lora_b->size(1);
+    TORCH_CHECK(lora_b->dim() == 2 && lora_b->is_contiguous() && lora_b->size(0) == N && R % 8 == 0, "lora_b must be contiguous [N, R], R % 8 == 0");
+    TORCH_CHECK(lora_b2.has_value() == wq2.has_value(), "a gate/up pair takes lora_b2, a single weight does not");
+    if (lora_b2.has_value()) { check_bf16(*lora_b2, "lora_b2"); TORCH_CHECK(lora_b2->sizes() == lora_b->sizes() && lora_b2->is_contiguous()); }
+    TORCH_CHECK(lora_u.has_value() && lora_u->is_cuda() && lora_u->scalar_type() == torch::kFloat32 && lora_u->is_contiguous() &&
+                lora_u->dim() == 2 && lora_u->size(0) >= x.size(0) && lora_u->size(1) == R * (wq2.has_value() ? 2 : 1),
+                "lora_u must be contiguous fp32 [T, R] ([T, 2R] for a pair)");
+    TORCH_CHECK(!out_fp32, "LoRA adapters run with bf16 output");
+    a.lora_u = lora_u->data_ptr<float>(); a.lora_b = lora_b->data_ptr(); a.lora_r = (int)R;
+    if (lora_b2.has_value()) a.lora_b2 = lora_b2->data_ptr();
   }
   return dense_linear(a, b200::kGemmQuant, x, residual, bias, act, softcap, out_fp32, out_, splits, signal_flag_ptr, signal_value);
 }
@@ -208,6 +223,19 @@ Tensor grouped_linear_q(const Tensor& x, const Tensor& wq, const Tensor& scales_
   LAUNCH_OK(b200::gemm_q_launch(a, b200::gemm_plan(a, b200::kGemmQuant, b200::sm_count()), cur_stream()));
   return out;
 }
+// LoRA shrink: fp32 u[T, R] = x[T, K] a[R, K]^T (R % 8 == 0), the first launch of an adapted quantised linear
+Tensor lora_shrink(const Tensor& x, const Tensor& a) {
+  check_bf16(x, "x"); check_rows(x, "x"); check_bf16(a, "a");
+  TORCH_CHECK(a.dim() == 2 && a.is_contiguous() && a.size(1) == x.size(1) && a.size(0) % 8 == 0 && x.size(1) % 8 == 0 &&
+              x.stride(0) % 8 == 0, "a must be contiguous [R, K] with R, K multiples of 8");
+  const c10::cuda::CUDAGuard guard(x.device());
+  Tensor u = torch::empty({x.size(0), a.size(0)}, x.options().dtype(torch::kFloat32));
+  if (x.size(0) == 0) return u;
+  LAUNCH_OK(b200::lora_shrink_launch(x.data_ptr(), x.stride(0), a.data_ptr(), (int)x.size(0), (int)x.size(1), (int)a.size(0),
+                                     u.data_ptr<float>(), cur_stream()));
+  return u;
+}
+
 bool gemm_q_supported(int64_t bits, int64_t group, int64_t k) { return b200::gemm_q_supported((int)bits, (int)group, (int)k); }
 
 // The launch plan the bindings above would use, from the GemmArgs fields the planner reads (kind: "bf16", "q" or "fp8").
@@ -756,7 +784,11 @@ PYBIND11_MODULE(TORCH_EXTENSION_NAME, m) {
         py::arg("signal_peers") = py::none(), py::arg("done_counter") = py::none(), py::arg("expected_rows") = 0,
         py::arg("expert_stride") = 0, py::arg("ep_arrive_ptr") = 0, py::arg("ep_seq") = py::none(), py::arg("ep_error_ptr") = 0,
         py::arg("ep_world") = 0, py::arg("ep_zero_other") = false);
-  m.def("linear_q", &linear_q);
+  m.def("linear_q", &linear_q, py::arg("x"), py::arg("wq"), py::arg("scales_t"), py::arg("biases_t"), py::arg("wq2"), py::arg("scales2_t"),
+        py::arg("biases2_t"), py::arg("bits"), py::arg("group"), py::arg("N"), py::arg("residual"), py::arg("bias"), py::arg("act"),
+        py::arg("softcap"), py::arg("out_fp32"), py::arg("out"), py::arg("splits"), py::arg("signal_flag_ptr"), py::arg("signal_value"),
+        py::arg("lora_u") = py::none(), py::arg("lora_b") = py::none(), py::arg("lora_b2") = py::none());
+  m.def("lora_shrink", &lora_shrink);
   m.def("grouped_linear_q", &grouped_linear_q);
   m.def("gemm_q_supported", &gemm_q_supported);
   m.def("gemm_plan", &gemm_plan, py::arg("kind"), py::arg("max_rows"), py::arg("n"), py::arg("k"), py::arg("pair") = false,

@@ -82,6 +82,13 @@ struct GemmArgs {
   int q_bits = 0, q_group = 64;
   const void* q_scales_t = nullptr; const void* q_biases_t = nullptr;
   const void* q_scales2_t = nullptr; const void* q_biases2_t = nullptr;
+  // LoRA adapter of a quantised launch (gemm_q_launch, bf16 output): the epilogue adds sum_j u[row, j] * lora_b[o, j] to the
+  // accumulator of feature o.  u = x A^T is fp32 [rows, lora_r] (lora_shrink_launch), for a pair [rows, 2 * lora_r] with the
+  // second weight's adapter in columns lora_r..; lora_b / lora_b2 are bf16 scale * B, [n, lora_r].  lora_r is a multiple of 8
+  // (0: no adapter).
+  const float* lora_u = nullptr;
+  const void* lora_b = nullptr; const void* lora_b2 = nullptr;
+  int lora_r = 0;
 };
 
 // Weight format of a launch: bf16, MLX affine int4 / int8 (dequantised in the kernel), MXFP8.
@@ -115,5 +122,7 @@ cudaError_t gemm_persistent_launch(const GemmArgs& a, const GemmPlan& plan, cuda
 bool gemm_q_supported(int bits, int group, int k);
 cudaError_t gemm_q_launch(const GemmArgs& a, const GemmPlan& plan, cudaStream_t stream);
 cudaError_t gemm_fp8_launch(const GemmArgs& a, const GemmPlan& plan, cudaStream_t stream);   // MXFP8 x MXFP8 -> bf16 / fp32 (gemm_fp8.cu)
+// LoRA shrink (lora.cu): u[T, R] = x[T, K] a[R, K]^T in fp32, bf16 inputs; R and K multiples of 8, rows 16-byte aligned
+cudaError_t lora_shrink_launch(const void* x, long long ld_x, const void* a, int T, int K, int R, float* u, cudaStream_t stream);
 
 }  // namespace b200

@@ -119,6 +119,46 @@ __device__ __forceinline__ float epi_value(const GemmParams& p, float g, float u
   return y;
 }
 
+// ---- LoRA term (adapted quantised launches)
+// A kernel parameter of its own, next to GemmParams, so the launches without an adapter keep their parameter layout.
+struct LoraParams {
+  const float* u;            // fp32 [rows, ld_u] = x A^T; a pair's second adapter starts at column r
+  const __nv_bfloat16* b;    // bf16 [n, r]: scale * B, one row per output feature
+  const __nv_bfloat16* b2;   // the pair's second weight
+  int r, ld_u;               // r: multiple of 8
+};
+
+__device__ __forceinline__ void lora_dot8(const float* u, const uint4 bw, float& acc) {
+  const float4 u0 = __ldg(reinterpret_cast<const float4*>(u)), u1 = __ldg(reinterpret_cast<const float4*>(u) + 1);
+  acc = fmaf(u0.x, bf16_lo(bw.x), acc); acc = fmaf(u0.y, bf16_hi(bw.x), acc);
+  acc = fmaf(u0.z, bf16_lo(bw.y), acc); acc = fmaf(u0.w, bf16_hi(bw.y), acc);
+  acc = fmaf(u1.x, bf16_lo(bw.z), acc); acc = fmaf(u1.y, bf16_hi(bw.z), acc);
+  acc = fmaf(u1.z, bf16_lo(bw.w), acc); acc = fmaf(u1.w, bf16_hi(bw.w), acc);
+}
+
+// Epilogue thread of feature f_glob, token rows row0 .. row0 + rows - 1 (rows <= 16): g[j] += sum_i u[row0 + j, i] * b[f_glob, i]
+// (and u / b2 for a pair's second accumulator).  Each thread streams its own contiguous row of B; the u loads are the same
+// address across the warp (broadcast).
+template <bool DUAL>
+__device__ __forceinline__ void lora_add16(const LoraParams& l, int n, int f_glob, int row0, int rows, float (&g)[16], float (&u)[16]) {
+  if (f_glob >= n) return;
+  const size_t fo = static_cast<size_t>(f_glob) * l.r;
+#pragma unroll 1
+  for (int i = 0; i < l.r; i += 8) {
+    const uint4 bw = __ldg(reinterpret_cast<const uint4*>(l.b + fo + i));
+    uint4 bw2;
+    if (DUAL) bw2 = __ldg(reinterpret_cast<const uint4*>(l.b2 + fo + i));
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      if (j < rows) {
+        const float* ur = l.u + static_cast<size_t>(row0 + j) * l.ld_u + i;
+        lora_dot8(ur, bw, g[j]);
+        if (DUAL) lora_dot8(ur + l.r, bw2, u[j]);
+      }
+    }
+  }
+}
+
 // ---- tile walk
 struct TileInfo {
   int n0, w_row, row_base, rows_valid, mt;   // rows_valid <= 0: the tile holds no token rows
@@ -226,9 +266,10 @@ __device__ __forceinline__ void write_rows(const GemmParams& p, const OutT* stg,
 
 // MMA warpgroup, one feature per thread: the tile's fp32 accumulator in shared memory (`acc`, [col][128 features], a pair's
 // second matrix at column BN) -> epilogue values -> staging tile [stg_rows(BN)][128] -> global, one staging tile of token rows
-// at a time.  Ends with the staging tile and the accumulator free again.
-template <int BN, bool DUAL, typename OutT>
-__device__ __forceinline__ void store_acc_tile(const GemmParams& p, const float* acc, OutT* stg, const TileInfo& ti) {
+// at a time.  Ends with the staging tile and the accumulator free again.  LORA: the adapter term joins the accumulator first.
+template <int BN, bool DUAL, typename OutT, bool LORA = false>
+__device__ __forceinline__ void store_acc_tile(const GemmParams& p, const float* acc, OutT* stg, const TileInfo& ti,
+                                               const LoraParams* lora = nullptr) {
   constexpr int STG_ROWS = stg_rows(BN);
   const int f_local = threadIdx.x;
   const float bias = feature_bias(p, ti.n0 + f_local);
@@ -244,6 +285,7 @@ __device__ __forceinline__ void store_acc_tile(const GemmParams& p, const float*
         g[j] = acc[(c + j) * kTileM + f_local];
         if (DUAL) u[j] = acc[(BN + c + j) * kTileM + f_local];
       }
+      if constexpr (LORA) lora_add16<DUAL>(*lora, p.n, ti.n0 + f_local, ti.row_base + c, ti.rows_valid - c, g, u);
 #pragma unroll
       for (int j = 0; j < 16; ++j) stage_store<OutT>(&stg[(c - c0 + j) * kTileM + f_local], epi_value<DUAL>(p, g[j], u[j], bias));
     }
@@ -273,10 +315,11 @@ __device__ __forceinline__ void publish_tiles_done(const GemmParams& p, unsigned
 
 // Workspace split-K route, on the MMA warpgroup once the tile's accumulator is in shared memory (`acc`, fp32 [col][128 features],
 // a pair's second matrix at column BN): write the raw partial, take the tile's ticket, and the last of its `splits` CTAs sums the
-// partials in split order, runs the epilogue through the staging tile `stg` [BN][128] and reports the tile as stored.
-template <int BN, bool DUAL, typename OutT>
+// partials in split order, runs the epilogue through the staging tile `stg` [BN][128] and reports the tile as stored.  LORA: the
+// adapter term joins the reduced sum (once per tile, not per split).
+template <int BN, bool DUAL, typename OutT, bool LORA = false>
 __device__ __forceinline__ void run_epilogue(const GemmParams& p, const float* acc, OutT* stg, uint32_t* flag_smem, const TileInfo& ti,
-                                             int split) {
+                                             int split, const LoraParams* lora = nullptr) {
   constexpr int kTileFloats = BN * (DUAL ? 2 : 1) * kTileM;
   const int f_local = threadIdx.x;   // 0..127: feature within the tile
   const int tile = (blockIdx.y * gridDim.x + blockIdx.x) * (gridDim.z / p.splits) + ti.mt;
@@ -326,6 +369,7 @@ __device__ __forceinline__ void run_epilogue(const GemmParams& p, const float* a
           if (DUAL) u[j] = (u[j] + b0[j]) + b1[j];
         }
       }
+      if constexpr (LORA) lora_add16<DUAL>(*lora, p.n, ti.n0 + f_local, ti.row_base + c, ti.rows_valid - c, g, u);
 #pragma unroll
       for (int j = 0; j < 16; ++j) stage_store<OutT>(&stg[(c + j) * kTileM + f_local], epi_value<DUAL>(p, g[j], u[j], bias));
     }

@@ -67,6 +67,15 @@ __device__ __forceinline__ void dequant_half_row(const uint8_t* packed_row, floa
 // Packed codes, scale and bias rows of each weight (the second set repeats the first without a pair) and the token tile.
 struct QMaps { CUtensorMap wq, wq2, s, b, s2, b2, x; };
 bool q_maps(const GemmArgs& a, int bn, QMaps* t);
+inline gemm::LoraParams lora_params(const GemmArgs& a) {
+  gemm::LoraParams l{};
+  l.u = a.lora_u;
+  l.b = static_cast<const __nv_bfloat16*>(a.lora_b);
+  l.b2 = static_cast<const __nv_bfloat16*>(a.lora_b2);
+  l.r = a.lora_r;
+  l.ld_u = a.w2 != nullptr ? 2 * a.lora_r : a.lora_r;
+  return l;
+}
 cudaError_t gemm_q_persistent_launch(const GemmArgs& a, const GemmPlan& plan, cudaStream_t stream);
 
 }  // namespace b200

@@ -37,13 +37,12 @@ __host__ __device__ constexpr int qp_num_stages(int BN, bool dual, int bits, int
 
 }  // namespace
 
-template <int BN, bool DUAL, typename OutT, int BITS>
-__global__ void __launch_bounds__(kQPThreads, 1)
-gemm_q_persistent_kernel(const __grid_constant__ CUtensorMap tmap_wq, const __grid_constant__ CUtensorMap tmap_wq2,
-                         const __grid_constant__ CUtensorMap tmap_s, const __grid_constant__ CUtensorMap tmap_b,
-                         const __grid_constant__ CUtensorMap tmap_s2, const __grid_constant__ CUtensorMap tmap_b2,
-                         const __grid_constant__ CUtensorMap tmap_x, const GemmParams p, const int group_kblocks, const int tiles_n,
-                         const int tiles_m, const int num_tiles) {
+// Kernel body; LORA adds the adapter term (LoraParams) in the epilogue.
+template <int BN, bool DUAL, typename OutT, int BITS, bool LORA>
+__device__ __forceinline__ void q_persistent_body(const CUtensorMap& tmap_wq, const CUtensorMap& tmap_wq2, const CUtensorMap& tmap_s,
+                                                  const CUtensorMap& tmap_b, const CUtensorMap& tmap_s2, const CUtensorMap& tmap_b2,
+                                                  const CUtensorMap& tmap_x, const GemmParams& p, const int group_kblocks,
+                                                  const int tiles_n, const int tiles_m, const int num_tiles, const LoraParams* lora) {
   constexpr int D = DUAL ? 2 : 1;
   constexpr int STAGES = qp_num_stages(BN, DUAL, BITS, sizeof(OutT));
   constexpr int STAGE_BYTES = qp_stage_bytes(BN, DUAL, BITS);
@@ -158,7 +157,7 @@ gemm_q_persistent_kernel(const __grid_constant__ CUtensorMap tmap_wq, const __gr
       acc_store_smem<BN>(acc, acc_smem, 0);
       if (DUAL) acc_store_smem<BN>(acc2, acc_smem, BN);
       named_bar_sync(1, kEpiThreads);
-      store_acc_tile<BN, DUAL, OutT>(p, acc_smem, stg, ti);
+      store_acc_tile<BN, DUAL, OutT, LORA>(p, acc_smem, stg, ti, lora);
       ++tc;
     }
     if (p.signal_flag != nullptr) {
@@ -195,18 +194,52 @@ gemm_q_persistent_kernel(const __grid_constant__ CUtensorMap tmap_wq, const __gr
       }
     }
   }
+}
 
+template <int BN, bool DUAL, typename OutT, int BITS>
+__global__ void __launch_bounds__(kQPThreads, 1)
+gemm_q_persistent_kernel(const __grid_constant__ CUtensorMap tmap_wq, const __grid_constant__ CUtensorMap tmap_wq2,
+                         const __grid_constant__ CUtensorMap tmap_s, const __grid_constant__ CUtensorMap tmap_b,
+                         const __grid_constant__ CUtensorMap tmap_s2, const __grid_constant__ CUtensorMap tmap_b2,
+                         const __grid_constant__ CUtensorMap tmap_x, const GemmParams p, const int group_kblocks, const int tiles_n,
+                         const int tiles_m, const int num_tiles) {
+  q_persistent_body<BN, DUAL, OutT, BITS, false>(tmap_wq, tmap_wq2, tmap_s, tmap_b, tmap_s2, tmap_b2, tmap_x, p, group_kblocks, tiles_n,
+                                                 tiles_m, num_tiles, nullptr);
+}
+
+// Adapted weights (bf16 output): the same kernel with the LoRA term in the epilogue.
+template <int BN, bool DUAL, int BITS>
+__global__ void __launch_bounds__(kQPThreads, 1)
+gemm_q_persistent_lora_kernel(const __grid_constant__ CUtensorMap tmap_wq, const __grid_constant__ CUtensorMap tmap_wq2,
+                              const __grid_constant__ CUtensorMap tmap_s, const __grid_constant__ CUtensorMap tmap_b,
+                              const __grid_constant__ CUtensorMap tmap_s2, const __grid_constant__ CUtensorMap tmap_b2,
+                              const __grid_constant__ CUtensorMap tmap_x, const GemmParams p, const int group_kblocks, const int tiles_n,
+                              const int tiles_m, const int num_tiles, const LoraParams lora) {
+  q_persistent_body<BN, DUAL, __nv_bfloat16, BITS, true>(tmap_wq, tmap_wq2, tmap_s, tmap_b, tmap_s2, tmap_b2, tmap_x, p, group_kblocks,
+                                                         tiles_n, tiles_m, num_tiles, &lora);
 }
 
 // ================================================================================================ host side
 namespace {
 
 template <int BN, bool DUAL, typename OutT, int BITS>
-cudaError_t qp_launch_one(const QMaps& t, const GemmParams& p, int gk, const GemmPlan& plan, cudaStream_t stream) {
+cudaError_t qp_launch_one(const QMaps& t, const GemmParams& p, int gk, const GemmPlan& plan, const LoraParams* lora, cudaStream_t stream) {
   constexpr int STAGES = qp_num_stages(BN, DUAL, BITS, sizeof(OutT));
   constexpr int smem = qp_dq(BN, DUAL) * kATileBytes * (DUAL ? 2 : 1) + STAGES * qp_stage_bytes(BN, DUAL, BITS) + acc_bytes(BN, DUAL) +
                        qp_staging_bytes(BN, sizeof(OutT)) + (2 * STAGES + 2 * qp_dq(BN, DUAL)) * 8 + 1024;
   static_assert(smem <= 227 * 1024, "shared memory budget exceeded");
+  if (lora != nullptr) {
+    if constexpr (std::is_same_v<OutT, __nv_bfloat16>) {
+      constexpr auto kern = gemm_q_persistent_lora_kernel<BN, DUAL, BITS>;
+      cudaError_t e = set_max_dynamic_smem_once<kern>(smem);
+      if (e != cudaSuccess) return e;
+      (void)launch_pdl(kern, plan.grid, dim3(kQPThreads), smem, stream, t.wq, t.wq2, t.s, t.b, t.s2, t.b2, t.x, p, gk, plan.tiles_n,
+                       plan.tiles_m, plan.num_tiles, *lora);
+      return cudaGetLastError();
+    } else {
+      return cudaErrorInvalidValue;   // adapters run with bf16 output only
+    }
+  }
   constexpr auto kern = gemm_q_persistent_kernel<BN, DUAL, OutT, BITS>;
   cudaError_t e = set_max_dynamic_smem_once<kern>(smem);
   if (e != cudaSuccess) return e;
@@ -226,11 +259,13 @@ cudaError_t gemm_q_persistent_launch(const GemmArgs& a, const GemmPlan& plan, cu
   QMaps t;
   if (!q_maps(a, plan.bn, &t)) return cudaErrorUnknown;
   const GemmParams p = gemm_params(a, plan);
+  const LoraParams lora = lora_params(a);
   const int gk = a.q_group / kBlockK;
   auto dispatch = [&](auto bits) {
     return dispatch_tile<kMaxBN, kMaxBNDual>(plan.bn, dual, a.out_fp32, [&](auto c) {
       using C = decltype(c);
-      return qp_launch_one<C::BN, C::DUAL, typename C::OutT, decltype(bits)::value>(t, p, gk, plan, stream);
+      return qp_launch_one<C::BN, C::DUAL, typename C::OutT, decltype(bits)::value>(t, p, gk, plan, a.lora_r > 0 ? &lora : nullptr,
+                                                                                    stream);
     });
   };
   if (a.q_bits == 4) return dispatch(std::integral_constant<int, 4>{});

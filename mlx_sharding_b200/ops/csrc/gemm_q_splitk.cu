@@ -38,12 +38,12 @@ __host__ __device__ constexpr int q_num_stages(int BN, bool dual, int bits, int 
 
 }  // namespace
 
-template <int BN, bool DUAL, typename OutT, int BITS>
-__global__ void __launch_bounds__(kQThreads, 1)
-gemm_swapab_q_kernel(const __grid_constant__ CUtensorMap tmap_wq, const __grid_constant__ CUtensorMap tmap_wq2,
-                     const __grid_constant__ CUtensorMap tmap_s, const __grid_constant__ CUtensorMap tmap_b,
-                     const __grid_constant__ CUtensorMap tmap_s2, const __grid_constant__ CUtensorMap tmap_b2,
-                     const __grid_constant__ CUtensorMap tmap_x, const GemmParams p, const int group_kblocks) {
+// Kernel body; LORA adds the adapter term (LoraParams) in the last CTA's reduction.
+template <int BN, bool DUAL, typename OutT, int BITS, bool LORA>
+__device__ __forceinline__ void q_splitk_body(const CUtensorMap& tmap_wq, const CUtensorMap& tmap_wq2, const CUtensorMap& tmap_s,
+                                              const CUtensorMap& tmap_b, const CUtensorMap& tmap_s2, const CUtensorMap& tmap_b2,
+                                              const CUtensorMap& tmap_x, const GemmParams& p, const int group_kblocks,
+                                              const LoraParams* lora) {
   constexpr int D = DUAL ? 2 : 1;
   constexpr int STAGES = q_num_stages(BN, DUAL, BITS, sizeof(OutT));
   constexpr int STAGE_BYTES = q_stage_bytes(BN, DUAL, BITS);
@@ -128,7 +128,7 @@ gemm_swapab_q_kernel(const __grid_constant__ CUtensorMap tmap_wq, const __grid_c
     acc_store_smem<BN>(acc, acc_smem, 0);
     if (DUAL) acc_store_smem<BN>(acc2, acc_smem, BN);
     named_bar_sync(1, kEpiThreads);
-    run_epilogue<BN, DUAL, OutT>(p, acc_smem, stg, flag_smem, ti, sk.split);
+    run_epilogue<BN, DUAL, OutT, LORA>(p, acc_smem, stg, flag_smem, ti, sk.split, lora);
   } else {
     // ============================================================== dequant producers: one weight row per thread
     const int r = threadIdx.x - kNumThreads;   // weight row of the tile
@@ -150,17 +150,47 @@ gemm_swapab_q_kernel(const __grid_constant__ CUtensorMap tmap_wq, const __grid_c
       if (lane == 0) mbar_arrive(&deq_bar[s]);
     }
   }
+}
 
+template <int BN, bool DUAL, typename OutT, int BITS>
+__global__ void __launch_bounds__(kQThreads, 1)
+gemm_swapab_q_kernel(const __grid_constant__ CUtensorMap tmap_wq, const __grid_constant__ CUtensorMap tmap_wq2,
+                     const __grid_constant__ CUtensorMap tmap_s, const __grid_constant__ CUtensorMap tmap_b,
+                     const __grid_constant__ CUtensorMap tmap_s2, const __grid_constant__ CUtensorMap tmap_b2,
+                     const __grid_constant__ CUtensorMap tmap_x, const GemmParams p, const int group_kblocks) {
+  q_splitk_body<BN, DUAL, OutT, BITS, false>(tmap_wq, tmap_wq2, tmap_s, tmap_b, tmap_s2, tmap_b2, tmap_x, p, group_kblocks, nullptr);
+}
+
+// Adapted weights (bf16 output): the same kernel with the LoRA term in the reduction's epilogue.
+template <int BN, bool DUAL, int BITS>
+__global__ void __launch_bounds__(kQThreads, 1)
+gemm_swapab_q_lora_kernel(const __grid_constant__ CUtensorMap tmap_wq, const __grid_constant__ CUtensorMap tmap_wq2,
+                          const __grid_constant__ CUtensorMap tmap_s, const __grid_constant__ CUtensorMap tmap_b,
+                          const __grid_constant__ CUtensorMap tmap_s2, const __grid_constant__ CUtensorMap tmap_b2,
+                          const __grid_constant__ CUtensorMap tmap_x, const GemmParams p, const int group_kblocks, const LoraParams lora) {
+  q_splitk_body<BN, DUAL, __nv_bfloat16, BITS, true>(tmap_wq, tmap_wq2, tmap_s, tmap_b, tmap_s2, tmap_b2, tmap_x, p, group_kblocks, &lora);
 }
 
 // ================================================================================================ host side
 namespace {
 
 template <int BN, bool DUAL, typename OutT, int BITS>
-cudaError_t q_launch_one(const QMaps& t, const GemmParams& p, int group_kblocks, const GemmPlan& plan, cudaStream_t stream) {
+cudaError_t q_launch_one(const QMaps& t, const GemmParams& p, int group_kblocks, const GemmPlan& plan, const LoraParams* lora,
+                         cudaStream_t stream) {
   constexpr int STAGES = q_num_stages(BN, DUAL, BITS, sizeof(OutT));
   constexpr int smem = STAGES * q_stage_bytes(BN, DUAL, BITS) + 3 * STAGES * 8 + 16 + 1024;
   static_assert(smem <= 227 * 1024, "shared memory budget exceeded");
+  if (lora != nullptr) {
+    if constexpr (std::is_same_v<OutT, __nv_bfloat16>) {
+      constexpr auto kern = gemm_swapab_q_lora_kernel<BN, DUAL, BITS>;
+      cudaError_t e = set_max_dynamic_smem_once<kern>(smem);
+      if (e != cudaSuccess) return e;
+      (void)launch_pdl(kern, plan.grid, dim3(kQThreads), smem, stream, t.wq, t.wq2, t.s, t.b, t.s2, t.b2, t.x, p, group_kblocks, *lora);
+      return cudaGetLastError();
+    } else {
+      return cudaErrorInvalidValue;   // adapters run with bf16 output only
+    }
+  }
   constexpr auto kern = gemm_swapab_q_kernel<BN, DUAL, OutT, BITS>;
   cudaError_t e = set_max_dynamic_smem_once<kern>(smem);
   if (e != cudaSuccess) return e;
@@ -204,6 +234,9 @@ bool gemm_q_supported(int bits, int group, int k) {
 
 cudaError_t gemm_q_launch(const GemmArgs& a, const GemmPlan& plan, cudaStream_t stream) {
   if (!gemm_q_supported(a.q_bits, a.q_group, a.k)) return cudaErrorNotSupported;
+  if (a.lora_r != 0 && (a.lora_r % 8 != 0 || a.lora_u == nullptr || a.lora_b == nullptr || (a.w2 != nullptr) != (a.lora_b2 != nullptr) ||
+                        a.out_fp32 || a.expert_offsets != nullptr))
+    return cudaErrorInvalidValue;
   if (plan.route == kRoutePersistent) return gemm_q_persistent_launch(a, plan, stream);
   const bool dual = a.w2 != nullptr;
   if (a.expert_offsets != nullptr && (a.n % kTileM) != 0) return cudaErrorInvalidValue;
@@ -214,11 +247,13 @@ cudaError_t gemm_q_launch(const GemmArgs& a, const GemmPlan& plan, cudaStream_t 
   QMaps t;
   if (!q_maps(a, plan.bn, &t)) return cudaErrorUnknown;
   const GemmParams p = gemm_params(a, plan);
+  const LoraParams lora = lora_params(a);
   const int gk = a.q_group / kBlockK;  // k-blocks per quantisation group (1 or 2)
   auto dispatch = [&](auto bits) {
     return dispatch_tile<kMaxBN, kMaxBNDual>(plan.bn, dual, a.out_fp32, [&](auto c) {
       using C = decltype(c);
-      return q_launch_one<C::BN, C::DUAL, typename C::OutT, decltype(bits)::value>(t, p, gk, plan, stream);
+      return q_launch_one<C::BN, C::DUAL, typename C::OutT, decltype(bits)::value>(t, p, gk, plan, a.lora_r > 0 ? &lora : nullptr,
+                                                                                   stream);
     });
   };
   if (a.q_bits == 4) return dispatch(std::integral_constant<int, 4>{});

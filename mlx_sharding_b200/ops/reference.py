@@ -66,11 +66,15 @@ def add_rmsnorm(x: torch.Tensor, residual: torch.Tensor, w: torch.Tensor, eps: f
 # ------------------------------------------------------------------------------------------ K3-K5, K8, K9, K12
 def linear(x: torch.Tensor, W: LinearWeight, residual: Optional[torch.Tensor] = None,
            out_dtype: Optional[torch.dtype] = None) -> torch.Tensor:
-    """``y = x @ W^T (+ bias) (+ residual)``; fp32 accumulate, single rounding at the end."""
+    """``y = x @ W^T (+ (x A^T) B_s^T) (+ bias) (+ residual)``; fp32 accumulate, single rounding at the end.  A packed weight's
+    LoRA adapter runs unfused, as in the CUDA backend's quantised GEMM epilogue."""
     if FAST_BASELINE and x.is_cuda and x.dtype != torch.float32:
-        y = F.linear(x, W.dense_cached(x.dtype)).float()  # cuBLAS bf16 path (baseline role)
+        y = F.linear(x, W.dense_cached(x.dtype)).float()  # cuBLAS bf16 path (baseline role; the adapter is folded in)
     else:
-        y = x.float() @ W.dense(torch.float32).t()
+        xf = x.float()
+        y = xf @ W.dense(torch.float32, fold_lora=False).t()
+        if W.has_lora:
+            y = y + (xf @ W.lora_a.float().t()) @ W.lora_b_scaled.float().t()
     if W.bias is not None:
         y = y + W.bias.float()
     if residual is not None:

@@ -24,6 +24,15 @@ class LinearWeight:
     bias: Optional[torch.Tensor] = None         # additive bias [N]
     group_size: int = 64
     bits: int = 4
+    # LoRA adapter kept unfused on a packed weight (utils/adapters.py): y += (x A^T) B_s^T, with A = ``lora_a`` bf16 [R, K] and
+    # B_s = ``lora_b_scaled`` = scale * B, bf16 [N, R] (one row per output feature).  Dense weights carry none: the adapter is
+    # folded into them at load.
+    lora_a: Optional[torch.Tensor] = None
+    lora_b_scaled: Optional[torch.Tensor] = None
+
+    @property
+    def has_lora(self) -> bool:
+        return self.lora_a is not None
 
     @property
     def is_quantized(self) -> bool:
@@ -43,8 +52,13 @@ class LinearWeight:
     def device(self):
         return (self.wq if self.is_quantized else self.weight).device
 
-    def dense(self, dtype: torch.dtype = torch.float32) -> torch.Tensor:
+    def dense(self, dtype: torch.dtype = torch.float32, fold_lora: bool = True) -> torch.Tensor:
+        """The weight in ``dtype``.  A packed weight's adapter is folded in (``W + B_s A`` in fp32, one rounding) unless
+        ``fold_lora`` is False: turning a weight dense ends its unfused adapter."""
         if self.is_quantized:
+            if self.has_lora and fold_lora:
+                w = quant.dequantize(self.wq, self.scales, self.biases, self.group_size, self.bits, torch.float32)
+                return (w + self.lora_b_scaled.float() @ self.lora_a.float()).to(dtype)
             return quant.dequantize(self.wq, self.scales, self.biases, self.group_size, self.bits, dtype)
         return self.weight.to(dtype)
 
@@ -67,11 +81,13 @@ class LinearWeight:
             return t.to(device=device)
 
         return LinearWeight(mv(self.weight, True), mv(self.wq, False), mv(self.scales, True),
-                            mv(self.biases, True), mv(self.bias, True), self.group_size, self.bits)
+                            mv(self.biases, True), mv(self.bias, True), self.group_size, self.bits,
+                            mv(self.lora_a, False), mv(self.lora_b_scaled, False))
 
     def nbytes(self) -> int:
         return sum(t.numel() * t.element_size()
-                   for t in (self.weight, self.wq, self.scales, self.biases, self.bias) if t is not None)
+                   for t in (self.weight, self.wq, self.scales, self.biases, self.bias, self.lora_a, self.lora_b_scaled)
+                   if t is not None)
 
     @staticmethod
     def from_state(sd: Dict[str, torch.Tensor], prefix: str, qcfg: Optional[Dict[str, int]] = None,
@@ -117,9 +133,22 @@ class LinearWeight:
                               torch.zeros(w.out_features, dtype=ws[0].bias.dtype if ws[0].bias is not None
                                           else torch.float32, device=w.device) for w in ws])
         if q:
+            la, lb = None, None
+            if any(w.has_lora for w in ws):
+                # block-diagonal adapter: A_cat = [A_1; A_2; ..] [sum r, K], B_cat [sum N, sum r] zero outside each module's
+                # block (a module without an adapter contributes an empty block) -- exact, one shrink and one GEMM
+                ref = next(w for w in ws if w.has_lora)
+                ranks = [w.lora_a.shape[0] if w.has_lora else 0 for w in ws]
+                la = torch.cat([w.lora_a for w in ws if w.has_lora], 0)
+                lb = torch.zeros(sum(w.out_features for w in ws), sum(ranks), dtype=ref.lora_b_scaled.dtype, device=ref.device)
+                n0 = r0 = 0
+                for w, r in zip(ws, ranks):
+                    if r:
+                        lb[n0:n0 + w.out_features, r0:r0 + r] = w.lora_b_scaled
+                    n0, r0 = n0 + w.out_features, r0 + r
             return LinearWeight(wq=torch.cat([w.wq for w in ws], dim), scales=torch.cat([w.scales for w in ws], dim),
                                 biases=torch.cat([w.biases for w in ws], dim), bias=bias,
-                                group_size=ws[0].group_size, bits=ws[0].bits)
+                                group_size=ws[0].group_size, bits=ws[0].bits, lora_a=la, lora_b_scaled=lb)
         return LinearWeight(weight=torch.cat([w.weight for w in ws], dim), bias=bias)
 
     def slice_out(self, start: int, end: int) -> "LinearWeight":
@@ -127,7 +156,8 @@ class LinearWeight:
         if self.is_quantized:
             return LinearWeight(wq=self.wq[sl], scales=self.scales[sl], biases=self.biases[sl],
                                 bias=None if self.bias is None else self.bias[start:end],
-                                group_size=self.group_size, bits=self.bits)
+                                group_size=self.group_size, bits=self.bits, lora_a=self.lora_a,
+                                lora_b_scaled=None if self.lora_b_scaled is None else self.lora_b_scaled[start:end])
         return LinearWeight(weight=self.weight[sl], bias=None if self.bias is None else self.bias[start:end])
 
     def slice_experts(self, lo: int, hi: int) -> "LinearWeight":

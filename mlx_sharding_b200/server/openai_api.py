@@ -139,7 +139,8 @@ def serve_expert_parallel_worker(args):
     from ..parallel.ep_serving import build_lockstep_group
     from ..utils.loader import load_model
 
-    model = load_model(args.model, device=_ep_device(args), expert_shard=(int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"])))
+    model = load_model(args.model, device=_ep_device(args), expert_shard=(int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"])),
+                       adapter_path=args.adapter_path)
     group = build_lockstep_group(model, args.kv_pages or 2048, args.page_size, max_seqs=args.max_batch)
     logging.info("expert-parallel worker rank %s ready", os.environ["RANK"])
     group.serve_forever()
@@ -249,9 +250,12 @@ class ModelProvider:
             ep = int(os.environ.get("WORLD_SIZE", "1")) > 1 and getattr(a, "expert_parallel", False)
             if ep and self.model_key is not None:
                 raise RuntimeError("model hot-swapping is not available in --expert-parallel mode")
+            # the LoRA adapter belongs to the --model checkpoint; a model picked per request is served as it is
+            adapter = getattr(a, "adapter_path", None) if path == a.model else None
             model = load_model(path, start_layer=None if ep else a.start_layer, end_layer=None if ep else a.end_layer,
                                device=_ep_device(a) if ep else getattr(a, "device", None),
-                               expert_shard=(int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"])) if ep else None)
+                               expert_shard=(int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"])) if ep else None,
+                               adapter_path=adapter)
             tokenizer = load_tokenizer(get_model_path(path), tok_cfg)
             if getattr(a, "use_default_chat_template", False) and tokenizer.chat_template is None:
                 tokenizer.chat_template = getattr(tokenizer, "default_chat_template", None)
@@ -611,7 +615,9 @@ def run(host: str, port: int, model_provider: ModelProvider, static_dir: str, ap
 def build_arg_parser() -> argparse.ArgumentParser:
     p = argparse.ArgumentParser(description="H100-native OpenAI-compatible HTTP server (mlx-sharding-api).")
     p.add_argument("--model", type=str, help="The path to the model weights, tokenizer, and config")
-    p.add_argument("--adapter-path", type=str, help="Optional path for trained adapter weights (accepted, unused)")
+    p.add_argument("--adapter-path", type=str,
+                   help="mlx_lm LoRA adapter directory (adapter_config.json + adapters.safetensors) applied to --model at load; "
+                        "every process of a pipeline applies it to the layers it holds (docs/SERVING.md)")
     p.add_argument("--host", type=str, default="127.0.0.1", help="Host for the HTTP server (default: 127.0.0.1)")
     p.add_argument("--port", type=int, default=8080, help="Port for the HTTP server (default: 8080)")
     p.add_argument("--trust-remote-code", action="store_true", help="Enable trusting remote code for tokenizer")
@@ -688,7 +694,7 @@ def main(argv=None):
 
             return serve_chain(args.model, args.start_layer, args.end_layer, args.device, None,
                                args.kv_pages or 2048, args.page_size, num_groups=world, max_tokens=args.max_prefill_tokens,
-                               max_seqs=args.max_batch, transport=args.transport)
+                               max_seqs=args.max_batch, transport=args.transport, adapter_path=args.adapter_path)
     needs_remote = args.end_layer is not None and world == 1 and not args.expert_parallel
     if args.model is not None and not needs_remote:
         try:

@@ -21,12 +21,12 @@ log = logging.getLogger("mlx_sharding_b200.shard_server")
 
 
 def serve(model_path: str, start_layer=None, end_layer=None, port: int = 0, device=None, dtype=None,
-          wire_dtype: str = "float16", num_pages: int = 512, page_size: int = 64, block: bool = True):
+          wire_dtype: str = "float16", num_pages: int = 512, page_size: int = 64, block: bool = True, adapter_path=None):
     """Compat mode: gRPC ``MLXTensorService`` for one stage (reference ``serve``)."""
     from ..parallel.grpc_compat import DTYPES, StageServicer, start_server
     from ..utils.loader import load_model
 
-    model = load_model(model_path, start_layer, end_layer, dtype=dtype, device=device)
+    model = load_model(model_path, start_layer, end_layer, dtype=dtype, device=device, adapter_path=adapter_path)
     servicer = StageServicer(model, num_pages=num_pages, page_size=page_size, wire_dtype=DTYPES[wire_dtype])
     server, bound = start_server(servicer, port)
     # the reference prints the port it picked (server.py:90); scripts parse this line
@@ -38,7 +38,8 @@ def serve(model_path: str, start_layer=None, end_layer=None, port: int = 0, devi
 
 
 def serve_chain(model_path: str, start_layer=None, end_layer=None, device=None, dtype=None, num_pages: int = 2048,
-                page_size: int = 64, num_groups=None, max_tokens: int = 2048, max_seqs: int = 64, transport: str = "auto"):
+                page_size: int = 64, num_groups=None, max_tokens: int = 2048, max_seqs: int = 64, transport: str = "auto",
+                adapter_path=None):
     """Native mode: this process is rank r > 0 of the chain pipeline (see parallel/pipeline.py)."""
     from ..config import ModelConfig
     from ..parallel.partition import balanced_split
@@ -54,7 +55,7 @@ def serve_chain(model_path: str, start_layer=None, end_layer=None, device=None, 
             spec = balanced_split(cfg, world)[rank]  # cost-balanced whole layers (LM head / dense layers weighted)
             start_layer, end_layer = spec.start_layer, spec.end_layer
     dev = device or (f"cuda:{torch.cuda.current_device()}" if torch.cuda.is_available() else "cpu")
-    model = load_model(model_path, start_layer, end_layer, dtype=dtype, device=dev)
+    model = load_model(model_path, start_layer, end_layer, dtype=dtype, device=dev, adapter_path=adapter_path)
     stage = StageExecutor(model, num_pages, page_size)
     # collective with the front end (openai_api.py / generate.py): same geometry on every rank
     ctl, plane = build_chain(stage, num_groups=num_groups, max_tokens=max_tokens, max_seqs=max_seqs, transport=transport)
@@ -67,6 +68,9 @@ def main(argv=None):
     parser.add_argument("--model", type=str, required=True, help="Path to the model or HF repo")
     parser.add_argument("-s", "--start-layer", type=int, default=None, help="Start layer index for model sharding")
     parser.add_argument("-e", "--end-layer", type=int, default=None, help="End layer index for model sharding")
+    parser.add_argument("--adapter-path", type=str, default=None,
+                        help="mlx_lm LoRA adapter directory; this stage applies it to the layers it loads (pass the same "
+                             "directory to every shard server and to mlx-sharding-api)")
     # extensions
     parser.add_argument("--port", type=int, default=0, help="gRPC port (0 = ephemeral, printed at start-up)")
     parser.add_argument("--device", type=str, default=None)
@@ -91,10 +95,11 @@ def main(argv=None):
         if args.rank is not None:
             os.environ.update(RANK=str(args.rank), WORLD_SIZE=str(args.world_size or 1),
                               MASTER_ADDR=args.master_addr, MASTER_PORT=str(args.master_port))
-        serve_chain(args.model, args.start_layer, args.end_layer, args.device, dtype, args.kv_pages or 2048, args.page_size)
+        serve_chain(args.model, args.start_layer, args.end_layer, args.device, dtype, args.kv_pages or 2048, args.page_size,
+                    adapter_path=args.adapter_path)
     else:
         serve(args.model, args.start_layer, args.end_layer, args.port, args.device, dtype, args.wire_dtype,
-              args.kv_pages or 512, args.page_size)
+              args.kv_pages or 512, args.page_size, adapter_path=args.adapter_path)
 
 
 if __name__ == "__main__":

@@ -361,3 +361,64 @@ def write_synthetic_checkpoint(path: str, config: Dict, dtype=torch.bfloat16, se
 
         write_byte_tokenizer(path, vocab_size=cfg.vocab_size)
     return path
+
+
+# ---------------------------------------------------------------------------------------------
+# Synthetic LoRA adapters (mlx_lm layout, see utils/adapters.py)
+# ---------------------------------------------------------------------------------------------
+def _module_shapes(cfg, i: int) -> Dict[str, Tuple[int, int]]:
+    """``module path -> (in, out)`` of the linear layers of block ``i`` that mlx_lm can adapt."""
+    H = cfg.hidden_size
+    if cfg.model_type == "deepseek_v2":
+        nh, qd = cfg.num_attention_heads, cfg.qk_nope_head_dim + cfg.qk_rope_head_dim
+        s = {"self_attn.kv_a_proj_with_mqa": (H, cfg.kv_lora_rank + cfg.qk_rope_head_dim),
+             "self_attn.kv_b_proj": (cfg.kv_lora_rank, nh * (cfg.qk_nope_head_dim + cfg.v_head_dim)),
+             "self_attn.o_proj": (nh * cfg.v_head_dim, H)}
+        if cfg.q_lora_rank is None:
+            s["self_attn.q_proj"] = (H, nh * qd)
+        else:
+            s.update({"self_attn.q_a_proj": (H, cfg.q_lora_rank), "self_attn.q_b_proj": (cfg.q_lora_rank, nh * qd)})
+        if cfg.is_moe_layer(i):
+            Is = cfg.moe_intermediate_size * (cfg.n_shared_experts or 0)
+            if Is:
+                s.update({"mlp.shared_experts.gate_proj": (H, Is), "mlp.shared_experts.up_proj": (H, Is),
+                          "mlp.shared_experts.down_proj": (Is, H)})
+        else:
+            I = cfg.intermediate_size
+            s.update({"mlp.gate_proj": (H, I), "mlp.up_proj": (H, I), "mlp.down_proj": (I, H)})
+        return s
+    hd, I = cfg.head_dim, cfg.intermediate_size
+    return {"self_attn.q_proj": (H, cfg.num_attention_heads * hd), "self_attn.k_proj": (H, cfg.num_key_value_heads * hd),
+            "self_attn.v_proj": (H, cfg.num_key_value_heads * hd), "self_attn.o_proj": (cfg.num_attention_heads * hd, H),
+            "mlp.gate_proj": (H, I), "mlp.up_proj": (H, I), "mlp.down_proj": (I, H)}
+
+
+def write_synthetic_adapter(path: str, cfg, rank: int = 8, scale: float = 20.0, num_layers: Optional[int] = None,
+                            modules: Optional[Iterable[str]] = None, seed: int = 0, zero_b: bool = False,
+                            std: float = 0.02) -> str:
+    """Write a random adapter in the mlx_lm layout for the last ``num_layers`` blocks (-1: all) of the model ``cfg`` (config dict or
+    ``ModelConfig``).  ``modules``: module paths inside a block (default: every adaptable linear, e.g. ``self_attn.q_proj``).
+    ``zero_b``: ``B = 0``, mlx_lm's initial state (the adapted model equals the base model)."""
+    from .adapters import CONFIG_FILE, WEIGHTS_FILE
+
+    cfg = cfg if isinstance(cfg, ModelConfig) else ModelConfig.from_dict(dict(cfg))
+    L = cfg.num_hidden_layers
+    num_layers = L if num_layers is None else int(num_layers)
+    gen = torch.Generator().manual_seed(seed)
+    tensors = {}
+    for i in range(L - num_layers if 0 < num_layers < L else 0, L):   # -1: every block, as mlx_lm writes it
+        shapes = _module_shapes(cfg, i)
+        for mod in (modules if modules is not None else shapes):
+            if mod not in shapes:
+                continue   # e.g. shared-expert modules on DeepSeek's dense layer
+            k_in, n_out = shapes[mod]
+            p = f"model.layers.{i}.{mod}"
+            tensors[p + ".lora_a"] = torch.randn(k_in, rank, generator=gen) * (1.0 / k_in ** 0.5)
+            tensors[p + ".lora_b"] = torch.zeros(rank, n_out) if zero_b else torch.randn(rank, n_out, generator=gen) * std
+    os.makedirs(path, exist_ok=True)
+    save_safetensors(os.path.join(path, WEIGHTS_FILE), tensors)
+    keys = sorted({m for m in (modules if modules is not None else _module_shapes(cfg, L - 1))})
+    with open(os.path.join(path, CONFIG_FILE), "w") as f:
+        json.dump({"fine_tune_type": "lora", "num_layers": num_layers,
+                   "lora_parameters": {"rank": rank, "scale": scale, "dropout": 0.0, "keys": keys}}, f, indent=2)
+    return path
