@@ -200,7 +200,7 @@ class StageModel:
             nonlocal total
             if isinstance(o, LinearWeight):
                 # (+ the concatenated A of an adapted gate/up pair, ops/b200.py::_lora_pair, once built)
-                for t in ((o.weight, o.wq, o.scales, o.biases, o.bias, o.lora_a, o.lora_b_scaled) + tuple(getattr(o, "_fp8", None) or ())
+                for t in ((o.weight, o.wq, o.scales, o.biases, o.bias, o.lora_a, o.lora_b_scaled) + (o.mxfp8 or ())
                           + tuple(getattr(o, "_lora_pair", ())[1:])):
                     if t is not None and t.data_ptr() not in seen:
                         seen.add(t.data_ptr())

@@ -72,8 +72,7 @@ class DeepseekV2Stage(StageModel):
         so a decode step needs no kv_b GEMM and attention runs on the cached 576-dim latent (``ops/csrc/mla_decode.cu``).  The
         original q / kv_b / o weights stay for prefill chunks, which decompress the context they attend to."""
         c = self.cfg
-        self._convert_quantized_for_b200()
-        self._fuse_shared_experts()
+        self._choose_weight_formats()
         if not (self.absorbed_mla and self.backend_name == "b200"):
             return
         if c.q_lora_rank is not None or not self.ops.mla_absorbed_supported(c.num_attention_heads, c.kv_lora_rank, c.qk_rope_head_dim):
@@ -208,76 +207,53 @@ class DeepseekV2Stage(StageModel):
         o_lat = O.paged_attention(torch.cat([q_abs, q[..., nope:]], -1), kpool, vpool, meta, c.attn_scale, 0.0)   # [T, nh, lr]
         return torch.einsum("thl,hvl->thv", o_lat.float(), wkv[:, nope:]).to(q.dtype).reshape(T, nh * vd)
 
-    def _convert_quantized_for_b200(self):
-        """Load-time policy for MLX 4/8-bit checkpoints on the CUDA backend (BASELINE config 2; off with MLXB200_FP8_EXPERTS=0, which
-        keeps every weight packed and dequantised in-kernel with exact MLX-affine semantics):
+    def _choose_weight_formats(self):
+        """The CUDA backend's weight formats, decided once at load from the checkpoint and the environment switch read below (and
+        nowhere else).  The switch selects block-scaled MXFP8 expert banks (``utils/quant.py::to_mxfp8``, run by wgmma e4m3 with
+        per-32 block scales in ``ops/csrc/gemm_fp8.cu``): ``1`` for every checkpoint, unset for MLX 4/8-bit ones (BASELINE config
+        2), ``0`` for none (packed banks keep the exact in-kernel MLX-affine dequant).  In a layer that takes FP8:
 
-        * routed + shared expert banks (93 % of the parameters) -> block-scaled MXFP8 (``utils/quant.py::to_mxfp8``), executed by
-          wgmma e4m3 with per-32 block scales (``ops/csrc/gemm_fp8.cu``); the shared experts are appended to the bank first;
-        * attention projections (7 %) -> bf16, so the absorbed-latent MLA path (folded weights, wgmma latent attention) applies;
+        * quantised attention projections (7 % of the parameters) -> bf16, so the absorbed-latent MLA path applies;
+        * routed + shared expert banks (93 %) -> MXFP8, when the hidden size and the expert width are multiples of 128;
         * embeddings, LM head, dense layer-0 MLP stay packed (in-kernel dequant GEMMs / gather).
 
-        With MLXB200_FP8_EXPERTS=1 the expert banks of a bf16 checkpoint are converted the same way."""
-        env = os.environ.get("MLXB200_FP8_EXPERTS", "")
-        if self.backend_name != "b200" or env == "0" or self.expert_shard is not None:
+        The shared experts are appended to a bf16 or MXFP8 bank as ``n_shared`` always-on experts (ids ``E .. E+n_shared-1``,
+        routing weight 1).  A SwiGLU MLP is separable along its intermediate dimension, so ``shared(x) = sum_j down_j(silu(gate_j x)
+        * up_j x)`` with ``j`` over ``n_shared`` slices of width ``moe_intermediate_size`` -- exactly the shape of a routed expert.
+        The two small dense GEMMs of the shared branch (latency-bound: ~37 us per layer for 35 MB of weights) disappear into the
+        persistent grouped GEMMs that already stream the bank at the HBM roofline; the router kernel emits the extra (id, 1.0)
+        columns itself.  A packed affine bank keeps its shared experts apart (appending them would re-quantise them), and an
+        expert-parallel stage (``expert_shard``) keeps every weight as loaded."""
+        if self.backend_name != "b200" or self.expert_shard is not None:
             return
-        from ..utils.quant import to_mxfp8
-
+        env = os.environ.get("MLXB200_FP8_EXPERTS", "")
         c = self.cfg
         ns, I, H = c.n_shared_experts or 0, c.moe_intermediate_size, c.hidden_size
         for w in self.layer_weights.values():
-            quantized = any(isinstance(v, LinearWeight) and v.is_quantized for v in w.values())
-            if not (quantized or env == "1"):
+            fp8 = env == "1" or (env != "0" and any(isinstance(v, LinearWeight) and v.is_quantized for v in w.values()))
+            if fp8:
+                for k in ("qkv_a", "q_a_kv_a", "q_b", "kv_b", "o"):
+                    if k in w and w[k].is_quantized:
+                        w[k] = LinearWeight(weight=w[k].dense(self.dtype).contiguous(), bias=w[k].bias)
+            if "router" not in w:
                 continue
-            for k in ("qkv_a", "q_a_kv_a", "q_b", "kv_b", "o"):
-                if k in w and w[k].is_quantized:
-                    w[k] = LinearWeight(weight=w[k].dense(self.dtype).contiguous(), bias=w[k].bias)
-            if "router" not in w or w.get("e_gate") is None or H % 128 or I % 128:
-                continue
-            fuse = bool(ns and "s_gate" in w and w["s_gate"].out_features == ns * I)
-
-            def bank(ek, sk, down=False):
-                parts = [w[ek].dense(torch.bfloat16)]
+            fp8 = fp8 and H % 128 == 0 and I % 128 == 0
+            ws = [w[k] for k in ("e_gate", "e_up", "e_down", "s_gate", "s_up", "s_down") if k in w]
+            fuse = ("s_gate" in w and w["s_gate"].out_features == ns * I and all(x.bias is None for x in ws)
+                    and (fp8 or not any(x.is_quantized for x in ws)))
+            for n in ("gate", "up", "down"):
+                bank = w["e_" + n]
                 if fuse:
-                    sd = w[sk].dense(torch.bfloat16)
-                    parts.append(sd.view(H, ns, I).permute(1, 0, 2) if down else sd.view(ns, I, H))
-                qs, sfs = zip(*(to_mxfp8(ch) for p_ in parts for ch in p_.split(8)))
-                out = LinearWeight()
-                out._fp8 = (torch.cat(qs).contiguous(), torch.cat(sfs).contiguous())
-                return out
-
-            w["e_gate"], w["e_up"], w["e_down"] = bank("e_gate", "s_gate"), bank("e_up", "s_up"), bank("e_down", "s_down", True)
+                    s = w.pop("s_" + n).dense(torch.bfloat16)
+                    s = s.view(H, ns, I).permute(1, 0, 2) if n == "down" else s.view(ns, I, H)
+                    bank = LinearWeight(weight=torch.cat([bank.dense(torch.bfloat16), s]))
+                w["e_" + n] = bank.to_mxfp8() if fp8 else bank
             if fuse:
-                for k in ("s_gate", "s_up", "s_down"):
-                    del w[k]
                 w["n_fused_shared"] = ns
 
-    def _fuse_shared_experts(self):
-        """CUDA backend, bf16 banks, whole banks on this rank: append DeepSeek's shared experts to the routed bank as ``n_shared``
-        always-on experts (ids ``E .. E+n_shared-1``, routing weight 1).  A SwiGLU MLP is separable along its intermediate dimension,
-        so ``shared(x) = sum_j down_j(silu(gate_j x) * up_j x)`` with ``j`` over ``n_shared`` slices of width ``moe_intermediate_size``
-        — exactly the shape of a routed expert.  The two small dense GEMMs of the shared branch (latency-bound: ~37 us per layer for
-        35 MB of weights) disappear into the persistent grouped GEMMs that already stream the bank at the HBM roofline; the router
-        kernel emits the extra (id, 1.0) columns itself."""
-        c = self.cfg
-        if not (self.backend_name == "b200" and self.expert_shard is None and c.n_shared_experts):
-            return
-        ns, I, H = c.n_shared_experts, c.moe_intermediate_size, c.hidden_size
-        for w in self.layer_weights.values():
-            if "router" not in w or "s_gate" not in w or w.get("e_gate") is None:
-                continue
-            ws = [w[k] for k in ("e_gate", "e_up", "e_down", "s_gate", "s_up", "s_down")]
-            if any(x.is_quantized or x.bias is not None or x.weight is None for x in ws) or w["s_gate"].weight.shape[0] != ns * I:
-                continue
-            w["e_gate"] = LinearWeight(weight=torch.cat([w["e_gate"].weight, w["s_gate"].weight.view(ns, I, H)], 0))
-            w["e_up"] = LinearWeight(weight=torch.cat([w["e_up"].weight, w["s_up"].weight.view(ns, I, H)], 0))
-            w["e_down"] = LinearWeight(weight=torch.cat([w["e_down"].weight, w["s_down"].weight.view(H, ns, I).permute(1, 0, 2)], 0))
-            for k in ("s_gate", "s_up", "s_down"):
-                del w[k]
-            w["n_fused_shared"] = ns
-
     def unfuse_shared_experts(self):
-        """Undo ``_fuse_shared_experts`` (expert parallelism shards the routed bank; the shared experts stay replicated)."""
+        """Undo the shared-expert append of ``_choose_weight_formats`` (expert parallelism shards the routed bank; the shared
+        experts stay replicated)."""
         c = self.cfg
         ns, I, H, E = c.n_shared_experts, c.moe_intermediate_size, c.hidden_size, c.n_routed_experts
         for w in self.layer_weights.values():
@@ -347,7 +323,7 @@ class DeepseekV2Stage(StageModel):
         ep = getattr(self, "ep_layers", {}).get(i)   # this layer's expert-parallel block (parallel/ep.py), if any
         rk = dict(top_k=c.num_experts_per_tok, method=c.topk_method, n_group=c.n_group or 1, topk_group=c.topk_group or 1,
                   scaling=c.routed_scaling_factor, norm_topk=c.norm_topk_prob)
-        if "router" in w and "s_gate" not in w and hasattr(O, "moe_block") and ep is None:
+        if "router" in w and "s_gate" not in w and self.backend_name == "b200" and ep is None:
             # CUDA backend, whole bank local, shared experts riding in the bank: the block is router -> grouped gate-up -> grouped
             # down -> combine, with BOTH RMSNorms around it folded in — the pre-MoE norm into the router kernel and the next layer's
             # input norm into the combine (decode batches; ops/b200.py::moe_block falls back to separate norm kernels otherwise)
@@ -368,7 +344,7 @@ class DeepseekV2Stage(StageModel):
             def shared_branch(normed):
                 if "s_gate" not in w:
                     return h, None
-                if hasattr(O, "run_aside"):
+                if self.backend_name == "b200":
                     hs = torch.empty_like(h)
                     return hs, O.run_aside(lambda: O.linear(O.gated_up(normed, w["s_gate"], w["s_up"], "silu"), w["s_down"], residual=h, out=hs))
                 return O.linear(O.gated_up(normed, w["s_gate"], w["s_up"], "silu"), w["s_down"], residual=h), None
@@ -387,7 +363,7 @@ class DeepseekV2Stage(StageModel):
                 # shared experts: h += down(silu(gate x) * up x).  Independent of the routed path until the final combine, so the
                 # CUDA backend runs the two GEMMs on a side stream (a parallel branch of the decode graph) while the main
                 # stream does router -> permutation / expert all-to-all -> expert GEMMs; the combine joins them.
-                if hasattr(O, "run_aside") and self.backend_name == "b200":
+                if self.backend_name == "b200":
                     hs, h_in = torch.empty_like(h), h   # result buffer allocated before the fork
                     join = O.run_aside(lambda: O.linear(O.gated_up(normed, w["s_gate"], w["s_up"], "silu"), w["s_down"],
                                                         residual=h_in, out=hs))

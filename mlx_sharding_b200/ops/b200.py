@@ -220,12 +220,14 @@ def paged_attention(q, kpool, vpool, meta: BatchMeta, scale: float, softcap: flo
 
 
 def moe_route(x, gate_w, top_k: int, method: str = "greedy", n_group: int = 1, topk_group: int = 1,
-              scaling: float = 1.0, norm_topk: bool = False, extra: int = 0):
-    """``extra``: always-on experts appended to the routed bank (ids E .. E+extra-1, weight 1.0) — see ``fuse_shared_experts``."""
+              scaling: float = 1.0, norm_topk: bool = False, extra: int = 0, scatter: tuple = ()):
+    """``extra``: always-on experts appended to the routed bank (ids E .. E+extra-1, weight 1.0) — see
+    ``models/deepseek_v2.py::_choose_weight_formats``.  ``scatter = (counts, stride, rows, norm_w, norm_eps)``: the scatter
+    layout of :func:`moe_block`; the kernel also places every (token, expert) pair's row and returns ``(idx, w, pair_row)``."""
     if method != "group_limited_greedy":
         n_group, topk_group = 1, 1
-    idx, w = C().moe_route(x, _bf16(gate_w), int(top_k), int(n_group), int(topk_group), float(scaling), bool(norm_topk), int(extra))
-    return idx, w
+    return tuple(C().moe_route(x, _bf16(gate_w), int(top_k), int(n_group), int(topk_group), float(scaling), bool(norm_topk),
+                               int(extra), *scatter))
 
 
 class _Join:
@@ -262,6 +264,34 @@ def run_aside(fn) -> _Join:
     return _Join(done)
 
 
+def _num_experts(W: LinearWeight) -> int:
+    return (W.mxfp8[0] if W.mxfp8 is not None else W.wq if W.is_quantized else W.weight).shape[0]
+
+
+def _expert_ffn(x, Wg: LinearWeight, Wu: LinearWeight, Wd: LinearWeight, act: str, rows: torch.Tensor, max_rows: int,
+                stride: int = 0, expected: int = 0) -> torch.Tensor:
+    """``down(act(gate x) * up x)`` of every expert over its rows of ``x``, as fp32 ``[rows, H]``: the grouped GEMM pair of the
+    bank's format (MXFP8, packed affine or bf16).  Row layout: ``rows`` = offsets ``[E + 1]`` into the compact permutation with
+    ``max_rows`` the largest group (``stride = 0``), or per-expert counts ``[E]`` of the scatter layout with ``max_rows = stride``
+    rows per expert segment and ``expected`` rows in all."""
+    c, a = C(), ACT_IDS[act]
+    if Wg.mxfp8 is not None:
+        # activations are quantised per 32-wide K block right before each GEMM (scatter rows beyond an expert's count are quantised
+        # too and never read); the FP8 GEMM applies both operands' block scales
+        xq, xsf = c.quant_mxfp8(x)
+        h = c.linear_fp8(xq, xsf, *Wg.mxfp8, *Wu.mxfp8, rows, max_rows, None, a, False, expected, stride)
+        hq, hsf = c.quant_mxfp8(h)
+        return c.linear_fp8(hq, hsf, *Wd.mxfp8, None, None, rows, max_rows, None, 0, True, expected, stride)
+    qg, qu, qd = _qpack(Wg), _qpack(Wu), _qpack(Wd)
+    if qg is not None and qu is not None and qd is not None:
+        E = Wg.wq.shape[0]
+        h = c.grouped_linear_q(x, *qg, *qu, Wg.bits, Wg.group_size, E, Wg.out_features, rows, max_rows, a, False)
+        return c.grouped_linear_q(h, *qd, None, None, None, Wd.bits, Wd.group_size, E, Wd.out_features, rows, max_rows, 0, True)
+    wg, wu, wd = _dense(Wg), _dense(Wu), _dense(Wd)
+    h = c.grouped_linear(x, wg, wu, rows, max_rows, a, False, None, None, None, expected, stride)
+    return c.grouped_linear(h, wd, None, rows, max_rows, 0, True, None, None, None, expected, stride)
+
+
 def moe_experts(x, idx, w, Wg: LinearWeight, Wu: LinearWeight, Wd: LinearWeight, act: str = "silu",
                 extra: Optional[torch.Tensor] = None, residual: Optional[torch.Tensor] = None,
                 out: Optional[torch.Tensor] = None, signal: Optional[Tuple[int, int]] = None, join: Optional[_Join] = None):
@@ -269,34 +299,8 @@ def moe_experts(x, idx, w, Wg: LinearWeight, Wu: LinearWeight, Wd: LinearWeight,
     weighted combine (+ residual [+ P2P store & flag])."""
     c = C()
     T, k = idx.shape
-    if fp8_experts_enabled(Wg) and x.shape[1] % 128 == 0:
-        (gq, gs), (uq, us), (dq, ds) = _fp8pack(Wg), _fp8pack(Wu), _fp8pack(Wd)
-        E = gq.shape[0]
-        offs, pair_row, xp = c.moe_permute(idx, x, E)
-        xq, xsf = c.quant_mxfp8(xp)
-        h = c.linear_fp8(xq, xsf, gq, gs, uq, us, offs, T, None, ACT_IDS[act], False, 0, 0)
-        hq, hsf = c.quant_mxfp8(h)
-        y = c.linear_fp8(hq, hsf, dq, ds, None, None, offs, T, None, 0, True, 0, 0)
-        if extra is not None:
-            residual = extra if residual is None else residual + extra
-        flag, val = signal if signal is not None else (0, 0)
-        if join is not None:
-            join.wait()
-        return c.moe_combine(y, pair_row, w, residual, out, int(k), int(flag), int(val))
-    qg, qu, qd = _qpack(Wg), _qpack(Wu), _qpack(Wd)
-    if qg is not None and qu is not None and qd is not None:
-        E = Wg.wq.shape[0]
-        offs, pair_row, xp = c.moe_permute(idx, x, E)
-        h = c.grouped_linear_q(xp, qg[0], qg[1], qg[2], qu[0], qu[1], qu[2], Wg.bits, Wg.group_size, E, Wg.out_features,
-                               offs, T, ACT_IDS[act], False)
-        y = c.grouped_linear_q(h, qd[0], qd[1], qd[2], None, None, None, Wd.bits, Wd.group_size, E, Wd.out_features, offs, T,
-                               0, True)
-    else:
-        wg, wu, wd = _dense(Wg), _dense(Wu), _dense(Wd)
-        E = wg.shape[0]
-        offs, pair_row, xp = c.moe_permute(idx, x, E)
-        h = c.grouped_linear(xp, wg, wu, offs, T, ACT_IDS[act], False)
-        y = c.grouped_linear(h, wd, None, offs, T, 0, True)
+    offs, pair_row, xp = c.moe_permute(idx, x, _num_experts(Wg))
+    y = _expert_ffn(xp, Wg, Wu, Wd, act, offs, T)
     if extra is not None:
         residual = extra if residual is None else residual + extra
     flag, val = signal if signal is not None else (0, 0)
@@ -308,33 +312,6 @@ def moe_experts(x, idx, w, Wg: LinearWeight, Wu: LinearWeight, Wd: LinearWeight,
 def quant_mxfp8(x: torch.Tensor):
     """bf16 activations ``[R, K]`` -> (e4m3 bytes, ue8m0 scales per 32 K-values): the B operand of the block-scaled FP8 GEMMs."""
     return C().quant_mxfp8(x)
-
-
-def _fp8pack(W: LinearWeight):
-    """MXFP8 form of a weight (``utils/quant.py::to_mxfp8``), built once on first use from the dense / dequantised values; the
-    source tensors (bf16 bank or packed MLX codes) are released — afterwards the weight lives in HBM as 1.03 bytes per parameter."""
-    f = getattr(W, "_fp8", None)
-    if f is None:
-        from ..utils.quant import to_mxfp8
-
-        src = W.dense(torch.bfloat16) if W.is_quantized else W.weight
-        qs, sfs = [], []
-        for chunk in (src.split(8) if src.dim() == 3 else [src]):     # bound the fp32 temporaries of the conversion
-            q, sf = to_mxfp8(chunk)
-            qs.append(q); sfs.append(sf)
-        f = W._fp8 = (torch.cat(qs).contiguous(), torch.cat(sfs).contiguous())
-        W.fp8_shape = tuple(src.shape)
-        W.weight = W.wq = W.scales = W.biases = None
-    return f
-
-
-def fp8_experts_enabled(W: LinearWeight) -> bool:
-    """Block-scaled FP8 expert banks.  The stage model converts at load (MLX 4/8-bit checkpoints by default, bf16 checkpoints with
-    MLXB200_FP8_EXPERTS=1; ``models/deepseek_v2.py::_convert_quantized_for_b200``); packed MLX weights handed to the ops directly
-    always take the exact in-kernel dequant GEMMs."""
-    if getattr(W, "_fp8", None) is not None:
-        return True                      # converted at load (models/deepseek_v2.py::_convert_quantized_for_b200)
-    return os.environ.get("MLXB200_FP8_EXPERTS", "") == "1" and not W.is_quantized   # explicit opt-in for bf16 banks used directly
 
 
 _scatter_bufs = {}
@@ -351,26 +328,19 @@ def moe_block(x, gate_w, route_kw: dict, Wg: LinearWeight, Wu: LinearWeight, Wd:
     the scatter path the router kernel normalises the row in shared memory (no norm kernel).  ``next_norm = (weight, eps)``: the
     block also returns ``rmsnorm(result) * weight`` (the next layer's input norm), fused into the combine kernel on the scatter
     path; the return value is then ``(result, normed)``.
-  Decode-sized batches with bf16 banks take the *scatter*
+  Decode-sized batches with bf16 or MXFP8 banks take the *scatter*
     path: the router kernel claims a slot per (token, expert) pair in the expert's fixed-stride segment and copies the token row
     there itself, the grouped GEMMs read per-expert row counts — route / counting sort / gather are ONE launch, the block is
     router -> grouped gate-up -> grouped down -> combine.  Larger batches (prefill) keep the compact counting-sort permutation."""
     c = C()
     T = x.shape[0]
-    fp8 = fp8_experts_enabled(Wg) and x.shape[1] % 128 == 0
-    quant = (Wg.is_quantized or Wu.is_quantized or Wd.is_quantized) and not fp8
-    if quant or T > SCATTER_MAX_TOKENS:
+    if Wg.is_quantized or Wu.is_quantized or Wd.is_quantized or T > SCATTER_MAX_TOKENS:
         if pre_norm is not None:
             x = rmsnorm(x, pre_norm[0], pre_norm[1])
         idx, wts = moe_route(x, gate_w, extra=extra, **route_kw)
         res = moe_experts(x, idx, wts, Wg, Wu, Wd, act, residual=residual, out=out, signal=signal)
         return res if next_norm is None else (res, rmsnorm(res, next_norm[0], next_norm[1]))
-    if fp8:
-        (gq, gs), (uq, us), (dq, ds) = _fp8pack(Wg), _fp8pack(Wu), _fp8pack(Wd)
-        E, H = gq.shape[0], x.shape[1]
-    else:
-        wg, wu, wd = _dense(Wg), _dense(Wu), _dense(Wd)
-        E, H = wg.shape[0], x.shape[1]
+    E, H = _num_experts(Wg), x.shape[1]
     stride = 64 if T <= 64 else SCATTER_MAX_TOKENS
     key = (x.device.index, E, H, stride)
     bufs = _scatter_bufs.get(key)
@@ -379,24 +349,10 @@ def moe_block(x, gate_w, route_kw: dict, Wg: LinearWeight, Wu: LinearWeight, Wd:
         bufs = _scatter_bufs[key] = (torch.zeros(E, dtype=torch.int32, device=x.device),
                                      torch.empty(E * stride, H, dtype=torch.bfloat16, device=x.device))
     counts, xs = bufs
-    rk = dict(route_kw)
-    method = rk.pop("method", "greedy")
-    if method != "group_limited_greedy":
-        rk["n_group"], rk["topk_group"] = 1, 1
     nw, ne = (_bf16(pre_norm[0]), float(pre_norm[1])) if pre_norm is not None else (None, 1e-6)
-    idx, wts, pair_row = c.moe_route(x, _bf16(gate_w), int(rk["top_k"]), int(rk["n_group"]), int(rk["topk_group"]), float(rk["scaling"]),
-                                     bool(rk["norm_topk"]), int(extra), counts, stride, xs, nw, ne)
+    idx, wts, pair_row = moe_route(x, gate_w, extra=extra, scatter=(counts, stride, xs, nw, ne), **route_kw)
     k = idx.shape[1]
-    if fp8:
-        # block-scaled FP8 experts: activations are quantised per 32-wide K block right before each GEMM (garbage rows beyond an
-        # expert's count are quantised too and never read); the FP8 GEMM applies both operands' block scales
-        xq, xsf = c.quant_mxfp8(xs)
-        h = c.linear_fp8(xq, xsf, gq, gs, uq, us, counts, stride, None, ACT_IDS[act], False, T * k, stride)
-        hq, hsf = c.quant_mxfp8(h)
-        y = c.linear_fp8(hq, hsf, dq, ds, None, None, counts, stride, None, 0, True, T * k, stride)
-    else:
-        h = c.grouped_linear(xs, wg, wu, counts, stride, ACT_IDS[act], False, None, None, None, T * k, stride)
-        y = c.grouped_linear(h, wd, None, counts, stride, 0, True, None, None, None, T * k, stride)
+    y = _expert_ffn(xs, Wg, Wu, Wd, act, counts, stride, stride, T * k)
     flag, val = signal if signal is not None else (0, 0)
     if next_norm is not None and signal is None and H <= 8192:
         normed = torch.empty(T, H, dtype=torch.bfloat16, device=x.device)

@@ -346,7 +346,8 @@ std::vector<Tensor> quant_mxfp8(const Tensor& x) {
   return {q, sf};
 }
 
-// Y = (xq * xsf) (wq * wsf)^T on the tensor cores (kind::mxf8f6f4.block_scale).  Dense: wq [N, K]; grouped: wq [E, N, K] with
+// Y = (xq * xsf) (wq * wsf)^T on wgmma e4m3, each 32-wide K block's product scaled by both operands' block scales in registers
+// (gemm_fp8.cu; sm_90 has no block-scaled MMA).  Dense: wq [N, K]; grouped: wq [E, N, K] with
 // expert_offsets (offsets, or per-expert counts when expert_stride > 0) exactly like grouped_linear.
 Tensor linear_fp8(const Tensor& xq, const Tensor& xsf, const Tensor& wq, const Tensor& wsf, const c10::optional<Tensor>& w2q,
                   const c10::optional<Tensor>& w2sf, const c10::optional<Tensor>& expert_offsets, int64_t max_rows,

@@ -8,7 +8,7 @@ dimension ``[E, N, K]`` is allowed for the stacked ``switch_mlp`` weights of Dee
 from __future__ import annotations
 
 from dataclasses import dataclass
-from typing import Dict, Optional
+from typing import Dict, Optional, Tuple
 
 import torch
 
@@ -29,6 +29,9 @@ class LinearWeight:
     # folded into them at load.
     lora_a: Optional[torch.Tensor] = None
     lora_b_scaled: Optional[torch.Tensor] = None
+    # block-scaled FP8 form (``quant.to_mxfp8``): (e4m3 codes uint8 [.., N, K], ue8m0 scales uint8 [.., N, K/32]).  A weight in
+    # this form carries nothing else (``to_mxfp8``).
+    mxfp8: Optional[Tuple[torch.Tensor, torch.Tensor]] = None
 
     @property
     def has_lora(self) -> bool:
@@ -87,7 +90,15 @@ class LinearWeight:
     def nbytes(self) -> int:
         return sum(t.numel() * t.element_size()
                    for t in (self.weight, self.wq, self.scales, self.biases, self.bias, self.lora_a, self.lora_b_scaled)
-                   if t is not None)
+                   + (self.mxfp8 or ()) if t is not None)
+
+    def to_mxfp8(self) -> "LinearWeight":
+        """This weight's bf16 values (dequantised, adapter folded in) in the ``mxfp8`` form: 1.03 bytes per parameter.  A stacked
+        ``[E, N, K]`` bank is converted 8 experts at a time, which bounds the fp32 temporaries and gives the same bytes as one
+        conversion (the scales are per 32 values of a row)."""
+        w = self.dense(torch.bfloat16)
+        qs, sfs = zip(*(quant.to_mxfp8(c) for c in (w.split(8) if w.dim() == 3 else [w])))
+        return LinearWeight(mxfp8=(torch.cat(qs).contiguous(), torch.cat(sfs).contiguous()))
 
     @staticmethod
     def from_state(sd: Dict[str, torch.Tensor], prefix: str, qcfg: Optional[Dict[str, int]] = None,
