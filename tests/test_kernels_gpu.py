@@ -157,47 +157,6 @@ def test_moe_route(B, method, n_group, topk_group, T):
     close(torch.gather(w1, 1, o1)[same], torch.gather(w2, 1, o2)[same], 1e-3, 2e-2)
 
 
-@pytest.mark.parametrize("T", [1, 64, 700])
-def test_moe_experts(B, T):
-    H, I, E, k = 2048, 1408, 64, 6
-    x = rnd(T, H)
-    gw = rnd(E, H, scale=0.05)
-    Wg = LinearWeight(weight=rnd(E, I, H, scale=0.03, seed=1))
-    Wu = LinearWeight(weight=rnd(E, I, H, scale=0.03, seed=2))
-    Wd = LinearWeight(weight=rnd(E, H, I, scale=0.03, seed=3))
-    idx, w = R.moe_route(x, gw, k)
-    res = rnd(T, H)
-    got = B.moe_experts(x, idx, w, Wg, Wu, Wd, "silu", residual=res)
-    dq = lambda w_: LinearWeight(weight=w_.dense(torch.bfloat16))
-    ref = R.moe_experts(x, idx, w, dq(Wg), dq(Wu), dq(Wd), "silu", residual=res)
-    close(got, ref, 5e-2, 2e-2)
-
-
-@pytest.mark.parametrize("T,extra", [(1, 0), (64, 2), (100, 2), (64, 0)])
-def test_moe_block_scatter_matches_permutation_path(B, T, extra):
-    """Scatter path (router claims slots + copies rows, grouped GEMMs on per-expert counts, combine resets the counters) ==
-    counting-sort permutation path, incl. the appended always-on (shared) experts; run twice: the counters must come back to 0."""
-    H, I, E, k = 2048, 1408, 64, 6
-    Et = E + extra
-    x = rnd(T, H)
-    gw = rnd(E, H, scale=0.05)
-    Wg = LinearWeight(weight=rnd(Et, I, H, scale=0.03, seed=1))
-    Wu = LinearWeight(weight=rnd(Et, I, H, scale=0.03, seed=2))
-    Wd = LinearWeight(weight=rnd(Et, H, I, scale=0.03, seed=3))
-    res = rnd(T, H)
-    rk = dict(top_k=k, method="greedy", n_group=1, topk_group=1, scaling=1.0, norm_topk=False)
-    idx, w = B.moe_route(x, gw, extra=extra, **rk)
-    assert idx.shape == (T, k + extra)
-    if extra:
-        assert (idx[:, k:] == torch.arange(E, Et, device=DEV, dtype=torch.int32)).all() and (w[:, k:] == 1).all()
-    ref = B.moe_experts(x, idx, w, Wg, Wu, Wd, "silu", residual=res)
-    for _ in range(2):
-        got = B.moe_block(x, gw, rk, Wg, Wu, Wd, "silu", residual=res, extra=extra)
-        close(got, ref, 2e-2, 1e-2)
-    torch.cuda.synchronize()
-    assert all(int(c.sum()) == 0 for c, _ in B._scatter_bufs.values())
-
-
 @pytest.mark.parametrize("T,extra", [(1, 0), (64, 2), (37, 2), (200, 2)])
 def test_moe_block_fused_norms(B, T, extra):
     """RMSNorm folded into the router kernel (pre-MoE norm) and into the combine kernel (next layer's input norm) == separate norm
@@ -327,15 +286,3 @@ def test_quantized_linear_in_kernel_dequant(B, bits, group, T):
     close(B.linear(x, W, residual=res, out_dtype=torch.float32), R.linear(x, dq(W), residual=res, out_dtype=torch.float32), 2e-2, 5e-3)
     Wu = _qweight(N, K, bits=bits, group=group, seed=2)
     close(B.gated_up(x, W, Wu, "silu"), R.gated_up(x, dq(W), dq(Wu), "silu"), 3e-2, 2e-2)
-
-
-def test_quantized_moe_experts(B):
-    H, I, E, k, T = 2048, 1408, 64, 6, 70
-    x = rnd(T, H)
-    Wg, Wu, Wd = _qweight(E, I, H, seed=1), _qweight(E, I, H, seed=2), _qweight(E, H, I, seed=3)
-    idx, w = R.moe_route(x, rnd(E, H, scale=0.05, seed=12), k)
-    res = rnd(T, H)
-    got = B.moe_experts(x, idx, w, Wg, Wu, Wd, "silu", residual=res)
-    dq = lambda w_: LinearWeight(weight=w_.dense(torch.bfloat16))
-    ref = R.moe_experts(x, idx, w, dq(Wg), dq(Wu), dq(Wd), "silu", residual=res)
-    close(got, ref, 5e-2, 2e-2)
